@@ -1,6 +1,6 @@
-"""bench.py -- CelebBasis training steps/sec (SD-v1 UNet 512^2, bs=1/GPU) on N B200s  (BASELINE.json metric).
+"""bench.py -- CelebBasis training steps/sec (SD-v1 UNet 512^2, bs=1/GPU) on N H100s  (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]                 # our arm (N>1: launched by torchrun)
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # our arm (N>1: launched by torchrun)
     python bench.py --impl reference --gpus N --steps K --warmup W      # the reference's CPU path (oracle port)
 
 One step = SURVEY.md §8 rows a1-a31 for one sample per GPU: VAE encode, CosFace R100 on the 2 face crops, celeb-basis
@@ -12,6 +12,9 @@ Output: ONE JSON line (rank 0).  `value` = whole-job steps/s with inputs residen
 `roofline` = tensor-pipe fraction of the dominant kernel (cb_gemm_kernel: every conv / linear / attention GEMM),
 measured live by replaying exactly the step's GEMM launches as their own CUDA graph under CUDA events;
 `cpu_baseline` = the oracle port of the reference step on this box's host cores.
+--dump-outputs DIR: after the timed steps, what the last timed step computed (loss, predicted noise, gradient of the
+trainable MLP, its weights after AdamW) as DIR/<name>.npy in float32.  Inputs and weights are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -36,11 +39,13 @@ def _peaks():
             p = json.load(f)
         return p, "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+        # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s -- never reached, and less on a
+        # power-limited card
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (dense BF16)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index=0):
         self.rows, self.proc, self.idx = [], None, gpu_index
@@ -203,10 +208,18 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------ our arm
+def dump_outputs(out_dir, arrays):
+    """Each tensor as out_dir/<name>.npy in float32 (the step's outputs are a few MB in all, far below 64 MB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy().astype(np.float32))
+
+
 def bench_config(world):
     """The workload description both arms print (identical dicts => the driver's same_config check holds)."""
     return {"workload": WORKLOAD, "per_gpu_batch": 1, "parallelism": f"dp{world}",
-            "l2": "inputs larger than L2: 2.1 GB of 16-bit weights + ~4 GB of activations are streamed every step (L2 = 126 MB)"}
+            "l2": "inputs larger than L2: 2.1 GB of 16-bit weights + ~4 GB of activations are streamed every step (L2 = 50 MB)"}
 
 
 def _file_sha1(path):
@@ -241,10 +254,11 @@ def run_ours(args):
 
     world, rank, local = cbd.init()
     json_out, sys.stdout = sys.stdout, sys.stderr       # stdout carries exactly one JSON line; library chatter -> stderr
+    torch.manual_seed(1000 + rank)                      # t / noise / posterior draws: identical inputs from run to run
     assert torch.cuda.is_available(), "bench.py needs a GPU (no CPU fallback in the product path)"
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    assert lib.load().cb_device_ok() == 1, "not an sm_100 device"
+    assert lib.load().cb_device_ok() == 1, "not an sm_90 (H100) device"
     assert world == args.gpus, f"--gpus {args.gpus} but WORLD_SIZE={world}"
     B = 1
 
@@ -318,6 +332,9 @@ def run_ours(args):
         clocks.start()
     ms_per_step = timed(one_step, args.steps) / args.steps
     value = world * B * 1000.0 / ms_per_step
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"loss": G.loss, "eps": eng.last["eps"], "grad": eng.grad, "mlp_weight": eng.W,
+                                         "mlp_bias": eng.b})
     # un-pipelined reference point: front end, then chain, back to back
     def serial_step():
         G.prefetch()
@@ -398,13 +415,13 @@ def run_ours(args):
         torch.cuda.synchronize()
         gemm_ms = e0.elapsed_time(e1) / reps
         peaks, src = _peaks()
-        peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
+        peak = float(peaks.get("bf16_tflops", 989.0))
         ach = flops / (gemm_ms * 1e-3) / 1e12
         traffic, traffic_src = _ncu_traffic()
-        roof = {"bound": "tensor", "kernel": "cb_gemm_kernel (tcgen05 GEMM / implicit-GEMM conv, all instantiations)",
+        roof = {"bound": "tensor", "kernel": "cb_gemm_kernel (wgmma GEMM / implicit-GEMM conv, all instantiations)",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
                 "traffic_source": traffic_src,
-                "peak_source": src + " bf16_tflops_sustained (kernel timed inside a long step)",
+                "peak_source": src + " bf16_tflops",
                 "launches_per_step": len(descs), "avg_launch_us": gemm_ms * 1e3 / len(descs),
                 "algorithmic_gflop_per_step": flops / 1e9, "gemm_ms_per_step": gemm_ms,
                 "gemm_share_of_serial_step": gemm_ms / ms_serial,
@@ -455,7 +472,7 @@ T2I_WORKLOAD = ("configs[3]: DDIM txt2img, 50 steps, 512x512, n_samples 8 per GP
 
 def t2i_config(world):
     return {"workload": T2I_WORKLOAD, "per_gpu_batch": 8, "parallelism": f"replicas x{world}",
-            "l2": "inputs larger than L2: 1.7 GB of UNet weights + ~6 GB of batch-16 activations per UNet call (L2 = 126 MB)"}
+            "l2": "inputs larger than L2: 1.7 GB of UNet weights + ~6 GB of batch-16 activations per UNet call (L2 = 50 MB)"}
 
 
 def run_txt2img(args):
@@ -560,11 +577,11 @@ def run_txt2img(args):
         torch.cuda.synchronize()
         gemm_ms = e0.elapsed_time(e1) / 5
         peaks, src = _peaks()
-        peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+        peak = float(peaks.get("bf16_tflops", 989.0))
         ach = flops / (gemm_ms * 1e-3) / 1e12
         roof = {"bound": "tensor", "kernel": "cb_gemm_kernel launches of ONE UNet forward at batch 16 (one DDIM step)",
                 "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
-                "peak_source": src + " bf16_tflops_sustained", "launches": len(descs), "gemm_ms_per_unet_call": gemm_ms,
+                "peak_source": src + " bf16_tflops", "launches": len(descs), "gemm_ms_per_unet_call": gemm_ms,
                 "algorithmic_gflop_per_unet_call": flops / 1e9,
                 "whole_job_tflops_per_gpu": 82.9 * B / (ms_batch * 1e-3),
                 "whole_job_frac": 82.9 * B / (ms_batch * 1e-3) / peak}
@@ -628,6 +645,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--skip-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32)")
     ap.add_argument("--workload", default="train", choices=["train", "txt2img"],
                     help="train = BASELINE.json metric (configs[1]); txt2img = configs[3] (images/s)")
     args = ap.parse_args()

@@ -1,7 +1,7 @@
-"""In-tree build of libcelebbasis_b200.so (sm_100a only) with explicit nvcc commands.
+"""In-tree build of libcelebbasis_b200.so (sm_90a only) with explicit nvcc commands.
 
 The shared object is the C-ABI declared in include/celebbasis_b200.h.  It is built next to this file
-so that it travels with the repo snapshot to the GPU box (a JIT cache under ~/.cache would not).
+so that the package is importable straight from the source tree (a JIT cache under ~/.cache would not be).
 """
 import hashlib
 import os
@@ -16,7 +16,7 @@ OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "libcelebbasis_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -80,7 +80,7 @@ def build(verbose=False, force=False):
             if r[2]:
                 sys.stderr.write(r[2])
     if rebuilt or not os.path.exists(LIB):
-        cmd = [nv, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs, "-lcudart"]
+        cmd = [nv, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs, "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,5 +1,5 @@
 """CLIP ViT-L/14 text transformer (12 pre-LN layers, 12 heads x 64, quick-GELU MLP, causal mask) forward and
-activation-gradient backward on the sm_100a kernels.
+activation-gradient backward on the sm_90a kernels.
 
 Mirrors what the reference runs through its patched HF forwards: ldm/modules/encoders/modules.py:345-406
 (text_encoder_forward: causal mask, encoder, final_layer_norm) and :302-342 (encoder_forward over

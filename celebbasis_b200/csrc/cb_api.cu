@@ -26,8 +26,8 @@ int device_sm_count() {
     static int n = 0;
     if (n == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     }
     return n;
 }
@@ -59,5 +59,10 @@ extern "C" int cb_device_ok(void) {
         cudaGetLastError();
         return 0;
     }
-    return major == 10 ? 1 : 0;
+    int minor = 0;
+    if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return (major == 9 && minor == 0) ? 1 : 0;   // sm_90a code runs on compute capability 9.0 only
 }

@@ -1,4 +1,4 @@
-// cb_attention_fwd — fused scaled-dot-product attention forward for sm_100a (flash style).
+// cb_attention_fwd — fused scaled-dot-product attention forward for sm_90a (flash style).
 //
 // Replaces the materialised `sim = einsum(q,k)*scale; attn = sim.softmax(-1); out = einsum(attn, v)` of
 // ldm/modules/attention.py:178-191 (and the CLIP layers' masked variant, encoders/modules.py:24-31): the
@@ -6,26 +6,24 @@
 // the caller asks for the probabilities (training keeps them for the backward pass).
 //
 // One CTA = 128 query rows of one (image, head):
-//   warp 0     : TMA producer -- Q once, then K_j / V_j blocks of 128 keys through a 2-stage mbarrier ring
-//   warp 1     : single-thread tcgen05.mma issuer: S_j = Q K_j^T into one of two TMEM score buffers,
-//                O += P_j V_j (V read MN-major straight from its [keys][d] layout) into the TMEM output tile
-//   warps 2..5 : one thread per query row: tcgen05.ld of the score row, online softmax (running max / sum in
-//                registers, exp2 with the scale folded in), rescale of the TMEM output tile when the max moves,
-//                P_j written as the next MMA's K-major SWIZZLE_128B A operand in shared memory;
-//                finally O / l -> HBM and logsumexp.
+//   warp 8        : TMA producer -- Q once, then K_j / V_j blocks of 64 keys through a 3-stage mbarrier ring
+//   warpgroups 0,1: query rows [0, 64) / [64, 128).  Per block: S_j = Q K_j^T with wgmma (fp32 in registers), online
+//                   softmax on the register fragment (running max / sum per row, exp2 with the scale folded in, row
+//                   reductions across the four lanes that share a row), P_j written as a K-major SWIZZLE_128B A tile in
+//                   shared memory, O += P_j V_j with wgmma (V read MN-major straight from its [keys][d] layout, O in
+//                   registers); finally O / l -> HBM and logsumexp.
 // Head dims 40 / 64 / 80 / 128 (any multiple of 8 up to 128): the tensor maps declare the head's d columns as the
 // K extent, so TMA zero-fills the rest of each 64-column box and the MMAs run on 16-column multiples.
 #include <string.h>
-
-#include <type_traits>
 
 #include "cb_common.cuh"
 
 namespace cb {
 
-constexpr int kAttnThreads = 192;
+constexpr int kAttnConsumers = 256;                  // two wgmma warpgroups
+constexpr int kAttnThreads = kAttnConsumers + 32;    // + the TMA producer warp
 constexpr int kBQ = 128;    // query rows per CTA
-constexpr int kBKV = 64;    // keys per block (64 scores per softmax thread keeps 2-4 CTAs resident per SM)
+constexpr int kBKV = 64;    // keys per block
 
 struct AttnParams {
     int nq, nk, heads, images;
@@ -41,8 +39,6 @@ struct AttnParams {
     void* P;                // optional probabilities [images*heads][nq][ldp] (same 16-bit dtype as the operands)
     long long ldp;
     int p_is_bf16;
-    unsigned idesc_s, idesc_o;
-    unsigned long long* dbg;      // profiling aid (tools/attn_timeline.py): per-CTA accumulated cycles of the softmax phases
 };
 
 template <int DBOX>  // number of 64-column boxes of the head dim (1: d <= 64, 2: d <= 128)
@@ -51,55 +47,53 @@ struct AttnCfg {
     static constexpr int kKBytes = DBOX * kBKV * 128;
     static constexpr int kVBytes = DBOX * kBKV * 128;
     static constexpr int kPBytes = kBQ * 128;              // 64 keys = one 128-byte chunk per query row
-    // K/V ring depth: a stage is re-requested only when the P.V of its previous block has retired, so with 2 stages the
-    // TMA round trip (~1.5 us under load) was exposed once per block; 4 stages keep ~3 blocks of K/V in flight.
     static constexpr int kStages = 3;
     static constexpr int kSmemBytes = kQBytes + kStages * (kKBytes + kVBytes) + 2 * kPBytes + 1024 + 256;   // two P buffers
-    static constexpr int kTmemCols = DBOX == 1 ? 128 : 256;   // S [0,64)  O [64, 64 + DBOX*64)
-    static constexpr int kMinBlocks = 2;
 };
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ uint32_t pack2(float a, float b, bool bf16) {
+    if (bf16) {
+        __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&h);
+    }
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+// two consecutive 16-bit values at (row r, column col) of a [128 rows][64 columns] K-major SWIZZLE_128B A tile
+__device__ __forceinline__ void st_a_pair(uint32_t tile, int r, int col, uint32_t v) {
+    const uint32_t dst = tile + r * 128 + ((((uint32_t)col >> 3) ^ ((uint32_t)r & 7u)) << 4) + (col & 7) * 2;
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(v) : "memory");
+}
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
 
 template <int DBOX>
-__global__ void __launch_bounds__(kAttnThreads, AttnCfg<DBOX>::kMinBlocks)
+__global__ void __launch_bounds__(kAttnThreads, 1)
 cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p) {
     using Cfg = AttnCfg<DBOX>;
+    constexpr int kSt = Cfg::kStages;
+    constexpr int NO = DBOX * 64;                 // output columns (zero-filled past d)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sQ = base;
     const uint32_t sKV = sQ + Cfg::kQBytes;                                 // stage s: K at sKV + s*(K+V), V after K
-    const uint32_t sP = sKV + Cfg::kStages * (Cfg::kKBytes + Cfg::kVBytes);
+    const uint32_t sP = sKV + kSt * (Cfg::kKBytes + Cfg::kVBytes);          // P of block j in buffer j & 1
     const uint32_t bars = sP + 2 * Cfg::kPBytes;
-    // barriers: q_full, kv_full[2], kv_empty[2], s_full[2], s_empty[2], p_full, pv_done ; then the TMEM slot
     const uint32_t bar_q = bars;
-    constexpr int kSt = Cfg::kStages;
     auto bar_kv_full = [&](int s) { return bars + 8u * (1 + s); };
     auto bar_kv_empty = [&](int s) { return bars + 8u * (1 + kSt + s); };
-    const uint32_t bar_s_full = bars + 8u * (1 + 2 * kSt);
-    const uint32_t bar_s_empty = bars + 8u * (2 + 2 * kSt);
-    // P is double-buffered (block j uses buffer j&1), each buffer with its own full / done barrier: the softmax of block
-    // j only waits for P.V of block j-2 (buffer reuse); it waits for block j-1 only when it must rescale the output tile.
-    auto bar_p_full = [&](int b) { return bars + 8u * (3 + 2 * kSt + b); };
-    auto bar_pv_done = [&](int b) { return bars + 8u * (5 + 2 * kSt + b); };
-    const uint32_t tmem_slot = bars + 8u * (7 + 2 * kSt);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * kBQ;
@@ -109,35 +103,22 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     const int nstat = p.two_pass ? nblk : 0;      // leading statistics-only virtual blocks
     const int nv = nstat + nblk;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ);
         tma_prefetch_desc(&tmK);
         tma_prefetch_desc(&tmV);
         mbar_init(bar_q, 1);
         for (int s = 0; s < kSt; ++s) {
             mbar_init(bar_kv_full(s), 1);
-            mbar_init(bar_kv_empty(s), 1);
-        }
-        mbar_init(bar_s_full, 1);
-        mbar_init(bar_s_empty, 128);
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(bar_p_full(b), 128);
-            mbar_init(bar_pv_done(b), 1);
+            mbar_init(bar_kv_empty(s), kAttnConsumers);
         }
         mbar_fence_init();
         fence_proxy_async_smem();
     }
-    if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-    __syncwarp();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
-    const uint32_t tS0 = tmem, tO = tmem + 64;
     pdl_sync();
 
-    if (warp == 0) {
+    if (warp == kAttnConsumers / 32) {
         if (lane == 0) {
             // ============================ TMA producer ============================
             mbar_arrive_expect_tx(bar_q, Cfg::kQBytes);
@@ -158,239 +139,152 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ============================ MMA issuer ============================
-            const int ks_qk = p.dpad16 / 16;
-            auto issue_S = [&](int vj) {
-                const int s = vj % kSt;
-                mbar_wait(bar_kv_full(s), (vj / kSt) & 1);
-                mbar_wait(bar_s_empty, (vj & 1) ^ 1u);      // softmax has copied the previous scores to registers
-                tc_fence_after();
-                const uint32_t aK = sKV + s * (Cfg::kKBytes + Cfg::kVBytes);
-                for (int k = 0; k < ks_qk; ++k) {
-                    const uint32_t offq = (k >> 2) * (kBQ * 128) + (k & 3) * 32;    // 64-col box, then 16-col step
-                    const uint32_t offk = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-                    umma_f16(tS0, umma_smem_desc_sw128(sQ + offq, 16, 1024), umma_smem_desc_sw128(aK + offk, 16, 1024),
-                             p.idesc_s, k > 0 ? 1u : 0u);
-                }
-                umma_commit(bar_s_full);
-                if (vj < nstat) umma_commit(bar_kv_empty(s));   // statistics pass: K stage is free once S is done
-            };
-            mbar_wait(bar_q, 0);
-            if (nv > 0) issue_S(0);
-            for (int vj = 0; vj < nv; ++vj) {
-                if (vj + 1 < nv) issue_S(vj + 1);          // next block's scores overlap this block's softmax
-                if (vj < nstat) continue;
-                const int fj = vj - nstat;
-                const int s = vj % kSt;
-                mbar_wait(bar_p_full(fj & 1), (fj >> 1) & 1);
-                tc_fence_after();
-                const uint32_t aV = sKV + s * (Cfg::kKBytes + Cfg::kVBytes) + Cfg::kKBytes;
-                for (int k = 0; k < kBKV / 16; ++k) {
-                    // A = P [128 rows][64 keys] K-major: 16-key step k
-                    const uint64_t ad = umma_smem_desc_sw128(sP + (fj & 1) * Cfg::kPBytes + k * 32, 16, 1024);
-                    // B = V [128 keys][d] read MN-major: 16 keys = 2 groups of 8 rows (SBO 1024), 64-col chunks at LBO
-                    const uint64_t bd = umma_smem_desc_sw128(aV + k * 2048, kBKV * 128, 1024);
-                    umma_f16(tO, ad, bd, p.idesc_o, (fj > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(bar_kv_empty(s));   // K_j / V_j stage reusable
-                umma_commit(bar_pv_done(fj & 1));       // this P buffer reusable, O stable up to block fj
-            }
+        return;
+    }
+
+    // ============================ consumers: 64 query rows per warpgroup ============================
+    const int wg = warp >> 2;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
+    const int cq = 2 * (lane & 3);                             // this thread's first column in every 8-column group
+    const bool bf16 = p.p_is_bf16 != 0;
+    const uint32_t qoff = static_cast<uint32_t>(wg) * 8192u;   // this warpgroup's 64 rows of a 128-row tile
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, inv_l[2] = {1.f, 1.f};
+    float o[NO / 2];
+#pragma unroll
+    for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
+    const int ks_qk = p.dpad16 / 16;
+    mbar_wait(bar_q, 0);
+    for (int vj = 0; vj < nv; ++vj) {
+        const bool full = vj >= nstat;
+        const int j = full ? vj - nstat : vj;
+        const int s = vj % kSt;
+        mbar_wait(bar_kv_full(s), (vj / kSt) & 1);
+        const uint32_t aK = sKV + s * (Cfg::kKBytes + Cfg::kVBytes), aV = aK + Cfg::kKBytes;
+        float sc[32];
+        wgmma_fence();
+        for (int k = 0; k < ks_qk; ++k) {
+            const uint32_t offq = (k >> 2) * (kBQ * 128) + qoff + (k & 3) * 32;    // 64-col box, then 16-col step
+            const uint32_t offk = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
+            wgmma_any<64, 0, 0>(bf16, sc, gmma_desc_sw128(sQ + offq, 16, 1024), gmma_desc_sw128(aK + offk, 16, 1024),
+                                k > 0 ? 1u : 0u);
         }
-    } else {
-        // ============================ softmax / epilogue: one thread per query row ============================
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const int qrow = q0 + r;
-        const bool row_ok = qrow < p.nq;
-        const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
-        float m = -INFINITY, l = 0.f;
-        const int et = threadIdx.x - 64;
-        const int ocols = DBOX * 64;
-        float inv_l = 1.f;
-        unsigned tph[6] = {0, 0, 0, 0, 0, 0};
-        const bool prof = p.dbg != nullptr && et == 0;
-        for (int vj = 0; vj < nv; ++vj) {
-            const bool full = vj >= nstat;
-            const int j = full ? vj - nstat : vj;
-            unsigned tc0 = 0, tc1;
-            if (prof) tc0 = (unsigned)clock64();
-            mbar_wait(bar_s_full, vj & 1);
-            tc_fence_after();
-            if (prof) { tc1 = (unsigned)clock64(); tph[0] += tc1 - tc0; tc0 = tc1; }
-            uint32_t sc[2][32];
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(sc);
+        if (!full) mbar_arrive(bar_kv_empty(s));          // statistics pass: the K stage is free once S is done
+        const int kbase = j * kBKV;
+        // masked keys -> -inf, then the row maxima on the raw scores (scale > 0 commutes with max)
+        float mx[2];
 #pragma unroll
-            for (int c = 0; c < 2; ++c) tmem_ld_32x32(tS0 + lane_off + c * 32, sc[c]);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(bar_s_empty);                       // the score tile may be overwritten by S_{vj+1}
-            if (prof) { tc1 = (unsigned)clock64(); tph[1] += tc1 - tc0; tc0 = tc1; }
-            const int kbase = j * kBKV;
+        for (int h = 0; h < 2; ++h) {
             int kvalid = min(kBKV, p.nk - kbase);
-            if (p.causal) kvalid = min(kvalid, qrow - kbase + 1);
-            // row max on the raw scores (scale > 0 commutes with max); masked blocks overwrite the invalid tail with
-            // -inf first, so the exp loop below is the same for both: e = ex2(fma(s, scale*log2e, -m))
-            float mx = -INFINITY;
-            if (kvalid >= kBKV) {
-                // four independent chains: a single running max is a 64-deep dependent FMNMX chain per block
-                float m4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+            if (p.causal) kvalid = min(kvalid, q0 + rl + 8 * h - kbase + 1);
+            float mh = -INFINITY;
 #pragma unroll
-                for (int c = 0; c < 2; ++c)
+            for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) m4[i & 3] = fmaxf(m4[i & 3], __uint_as_float(sc[c][i]));
-                mx = fmaxf(fmaxf(m4[0], m4[1]), fmaxf(m4[2], m4[3]));
-            } else {
+                for (int c = 0; c < 2; ++c) {
+                    float& v = sc[4 * jj + 2 * h + c];
+                    if (jj * 8 + cq + c >= kvalid) v = -INFINITY;
+                    mh = fmaxf(mh, v);
+                }
+            mx[h] = quad_max(mh) * p.scale_log2e;
+        }
+        const bool online = !(p.two_pass && full);      // running max / sum still being built
+        float m_use[2];
 #pragma unroll
-                for (int c = 0; c < 2; ++c)
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const float v = (c * 32 + i < kvalid) ? __uint_as_float(sc[c][i]) : -INFINITY;
-                        sc[c][i] = __float_as_uint(v);
-                        mx = fmaxf(mx, v);
-                    }
-            }
-            mx *= p.scale_log2e;
-            if (prof) { tc1 = (unsigned)clock64(); tph[2] += tc1 - tc0; tc0 = tc1; }
-            const bool online = !(p.two_pass && full);      // running max / sum still being built
-            float m_use = m;
-            // wait until P.V of block jj has retired (barrier of its P buffer, phase jj>>1)
-            auto wait_pv = [&](int jj) { mbar_wait(bar_pv_done(jj & 1), (jj >> 1) & 1); tc_fence_after(); };
+        for (int h = 0; h < 2; ++h) {
             if (online) {
                 // Lazy rescale: the reference maximum only moves when the block maximum exceeds it by more than 2^8
-                // (probabilities stay <= 256, exact in fp16/fp32), so the TMEM output tile is rescaled -- and the previous
-                // P.V waited for -- a handful of times per row instead of nearly every block.
-                const float m_new = fmaxf(m, mx);
+                // (probabilities stay <= 256, exact in fp16/fp32).
+                const float m_new = fmaxf(m[h], mx[h]);
                 float corr = 1.f;
-                if (m == -INFINITY) {
-                    m = m_new;                               // first block: nothing accumulated yet (l = 0, O untouched)
-                } else if (m_new > m + 8.f) {
-                    corr = fast_exp2(m - m_new);
-                    m = m_new;
+                if (m[h] == -INFINITY) {
+                    m[h] = m_new;                            // first block: nothing accumulated yet (l = 0, O zero)
+                } else if (m_new > m[h] + 8.f) {
+                    corr = fast_exp2(m[h] - m_new);
+                    m[h] = m_new;
                 }
-                l *= corr;
-                if (full) {
-                    const bool need = __any_sync(0xffffffffu, j > 0 && corr != 1.f);   // tcgen05.ld/st are warp-collective
-                    if (need) {
-                        wait_pv(j - 1);                     // the previous P.V must be complete before O is rescaled
-                        for (int c = 0; c * 32 < ocols; ++c) {
-                            uint32_t o[32];
-                            tmem_ld_32x32(tO + lane_off + c * 32, o);
-                            tmem_ld_wait();
+                l[h] *= corr;
+                if (full && corr != 1.f) {
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * corr);
-                            tmem_st_32x32(tO + lane_off + c * 32, o);
-                        }
-                        tmem_st_wait();
-                        tc_fence_before();
-                    }
+                    for (int jj = 0; jj < NO / 8; ++jj) { o[4 * jj + 2 * h] *= corr; o[4 * jj + 2 * h + 1] *= corr; }
                 }
             }
-            m_use = (m == -INFINITY) ? 0.f : m;             // (fully masked so far: the exponent argument stays -inf)
-            if (full && j > 1) wait_pv(j - 2);              // P buffer j&1 was last read by the P.V of block j-2
-            if (prof) { tc1 = (unsigned)clock64(); tph[3] += tc1 - tc0; tc0 = tc1; }
-            if (!full) {                                    // statistics pass: accumulate the row sum only
+            m_use[h] = (m[h] == -INFINITY) ? 0.f : m[h];  // (fully masked so far: the exponent argument stays -inf)
+        }
+        if (!full) {                                    // statistics pass: accumulate the row sums only
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
                 float rs = 0.f;
 #pragma unroll
-                for (int c = 0; c < 2; ++c)
+                for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) rs += fast_exp2(fmaf(__uint_as_float(sc[c][i]), p.scale_log2e, -m_use));
-                l += rs;
-                if (vj == nstat - 1) inv_l = l > 0.f ? 1.f / l : 0.f;
-                continue;
+                    for (int c = 0; c < 2; ++c) rs += fast_exp2(fmaf(sc[4 * jj + 2 * h + c], p.scale_log2e, -m_use[h]));
+                l[h] += rs;
+                if (vj == nstat - 1) {
+                    l[h] = quad_sum(l[h]);
+                    inv_l[h] = l[h] > 0.f ? 1.f / l[h] : 0.f;
+                }
             }
-            // P = exp2(s - m) (normalised by 1/l in two-pass mode): swizzled K-major A tile in smem (+ optional HBM copy)
-            float rs4[4] = {0.f, 0.f, 0.f, 0.f};      // independent partial row sums (no 64-deep FADD chain)
-            uint16_t* prow = (p.P && row_ok)
-                                 ? reinterpret_cast<uint16_t*>(p.P) +
-                                       ((static_cast<long long>(img) * p.heads + head) * p.nq + qrow) * p.ldp + kbase
+            continue;
+        }
+        // P = exp2(s - m) (normalised by 1/l in two-pass mode): swizzled K-major A tile in smem (+ optional HBM copy)
+        const uint32_t tile = sP + (j & 1) * Cfg::kPBytes;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int qrow = q0 + rl + 8 * h;
+            uint32_t* prow = (p.P && qrow < p.nq)
+                                 ? reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.P) +
+                                                               ((static_cast<long long>(img) * p.heads + head) * p.nq + qrow) * p.ldp + kbase + cq)
                                  : nullptr;
-            const float pscale = p.two_pass ? inv_l : 1.f;
-            auto write_p = [&](auto scaled) {
+            const float pscale = p.two_pass ? inv_l[h] : 1.f;
+            float rs = 0.f;
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float e[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        e[i] = fast_exp2(fmaf(__uint_as_float(sc[c][g * 8 + i]), p.scale_log2e, -m_use));
-                        if (decltype(scaled)::value) e[i] *= pscale;
-                        rs4[i & 3] += e[i];
-                    }
-                    uint4 pk;
-                    if (p.p_is_bf16) {
-                        __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(e[2 * i], e[2 * i + 1]);
-                    } else {
-                        __half2* h = reinterpret_cast<__half2*>(&pk);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(e[2 * i], e[2 * i + 1]);
-                    }
-                    const int key8 = c * 4 + g;                               // 8-key group 0..7
-                    const uint32_t dst = sP + (j & 1) * Cfg::kPBytes + r * 128 + ((key8 ^ (r & 7)) << 4);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk.x), "r"(pk.y), "r"(pk.z),
-                                 "r"(pk.w)
-                                 : "memory");
-                    if (prow && kbase + key8 * 8 < p.ldp) *reinterpret_cast<uint4*>(prow + key8 * 8) = pk;
-                }
+            for (int jj = 0; jj < 8; ++jj) {
+                const float e0 = fast_exp2(fmaf(sc[4 * jj + 2 * h], p.scale_log2e, -m_use[h])) * pscale;
+                const float e1 = fast_exp2(fmaf(sc[4 * jj + 2 * h + 1], p.scale_log2e, -m_use[h])) * pscale;
+                rs += e0 + e1;
+                const uint32_t v = pack2(e0, e1, bf16);
+                st_a_pair(tile, rl + 8 * h, jj * 8 + cq, v);
+                if (prow && kbase + jj * 8 < p.ldp) prow[jj * 4] = v;
             }
-            };
-            if (p.two_pass) write_p(std::true_type{}); else write_p(std::false_type{});
-            if (online) l += (rs4[0] + rs4[1]) + (rs4[2] + rs4[3]);
-            if (prof) { tc1 = (unsigned)clock64(); tph[4] += tc1 - tc0; tc0 = tc1; }
-            fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core (async proxy)
-            tc_fence_before();
-            mbar_arrive(bar_p_full(j & 1));
-            if (prof) { tc1 = (unsigned)clock64(); tph[5] += tc1 - tc0; }
+            if (online) l[h] += rs;
         }
-        if (prof) {
-            unsigned long long* d = p.dbg + 8ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
+        fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core (async proxy)
+        named_bar(1 + wg, 128);         // this warpgroup's 64 rows of P are complete
+        wgmma_fence_regs(o);
+        wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 6; ++i) d[i] = tph[i];
-            d[6] = nv;
+        for (int k = 0; k < kBKV / 16; ++k) {
+            // A = P [64 rows][64 keys] K-major: 16-key step k;  B = V [64 keys][d] MN-major: 16 keys = 2 groups of 8 rows
+            // (SBO 1024), 64-col chunks at LBO
+            wgmma_any<NO, 0, 1>(bf16, o, gmma_desc_sw128(tile + qoff + k * 32, 16, 1024),
+                                gmma_desc_sw128(aV + k * 2048, kBKV * 128, 1024), 1u);
         }
-        // ---- epilogue: O / l, logsumexp ----
-        if (nblk > 1) mbar_wait(bar_pv_done((nblk - 2) & 1), ((nblk - 2) >> 1) & 1);
-        if (nblk > 0) mbar_wait(bar_pv_done((nblk - 1) & 1), ((nblk - 1) >> 1) & 1);
-        tc_fence_after();
-        const float inv = p.two_pass ? 1.f : (l > 0.f ? 1.f / l : 0.f);
-        if (row_ok && p.lse && et >= 0)
-            p.lse[(static_cast<long long>(img) * p.heads + head) * p.nq + qrow] = (m + log2f(l)) * 0.6931471805599453f;
-        for (int c = 0; c * 32 < ocols; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(tO + lane_off + c * 32, o);
-            tmem_ld_wait();
-            if (row_ok) {
-                const long long orow = (static_cast<long long>(img) * p.nq + qrow) * p.ldo + static_cast<long long>(head) * p.d;
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        mbar_arrive(bar_kv_empty(s));   // K_j / V_j stage reusable
+    }
+    // ---- epilogue: O / l, logsumexp ----
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const int col = c * 32 + g * 8;
-                    if (col < p.d) {
-                        float f[8];
+    for (int h = 0; h < 2; ++h) {
+        if (!p.two_pass) l[h] = quad_sum(l[h]);
+        const int qrow = q0 + rl + 8 * h;
+        if (qrow >= p.nq) continue;
+        const float inv = p.two_pass ? 1.f : (l[h] > 0.f ? 1.f / l[h] : 0.f);
+        if (p.lse && (lane & 3) == 0)
+            p.lse[(static_cast<long long>(img) * p.heads + head) * p.nq + qrow] = (m[h] + log2f(l[h])) * 0.6931471805599453f;
+        uint16_t* orow = reinterpret_cast<uint16_t*>(p.O) + (static_cast<long long>(img) * p.nq + qrow) * p.ldo +
+                         static_cast<long long>(head) * p.d;
 #pragma unroll
-                        for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(o[g * 8 + i]) * inv;
-                        uint4 pk;
-                        if (p.o_dtype == CB_BF16) {
-                            __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-                        } else {
-                            __half2* h = reinterpret_cast<__half2*>(&pk);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
-                        }
-                        *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.O) + orow + col) = pk;
-                    }
-                }
-            }
+        for (int jj = 0; jj < NO / 8; ++jj) {
+            const int col = jj * 8 + cq;
+            if (col < p.d)
+                *reinterpret_cast<uint32_t*>(orow + col) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, p.o_dtype == CB_BF16);
         }
     }
-    __syncwarp();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem);
 }
 
 int make_tmap(CUtensorMap* out, int dtype, int rank, const void* ptr, const uint64_t* dims,
@@ -406,7 +300,7 @@ static int launch_attn(const CUtensorMap& q, const CUtensorMap& k, const CUtenso
         CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
         done = true;
     }
-CB_LAUNCH((kern), grid, kAttnThreads, Cfg::kSmemBytes, st, q, k, v, p);
+    CB_LAUNCH((kern), grid, kAttnThreads, Cfg::kSmemBytes, st, q, k, v, p);
     CB_CUDA(cudaGetLastError());
     count_launches(1);
     return 0;
@@ -417,9 +311,9 @@ CB_LAUNCH((kern), grid, kAttnThreads, Cfg::kSmemBytes, st, q, k, v, p);
 // Backward.  Two launches of one kernel template, both without atomics and without the (heads x N x N) tensors:
 //   MODE 0 (dQ)    : CTA = 128 query rows.  X1 = Q, X2 = dO stationary; per 64-key block Y1 = K_j, Y2 = V_j.
 //   MODE 1 (dK,dV) : CTA = 128 key rows.    X1 = K, X2 = V  stationary; per 64-query block Y1 = Q_j, Y2 = dO_j.
-// Every block: T1 = X1 Y1^T (scores, or their transpose) and T2 = X2 Y2^T (dP, or its transpose) into TMEM;
-// one thread per stationary row rebuilds P = exp2(T1*scale*log2e - lse*log2e) and dS = P o (T2 - delta) * scale with the
-// forward's log-sum-exp and delta = rowsum(dO o O) (indexed by row in MODE 0, by column in MODE 1) and writes them as
+// Every block, per warpgroup of 64 stationary rows: T1 = X1 Y1^T (scores, or their transpose) and T2 = X2 Y2^T (dP, or
+// its transpose) with wgmma into registers; P = exp2(T1*scale*log2e - lse*log2e) and dS = P o (T2 - delta) * scale with
+// the forward's log-sum-exp and delta = rowsum(dO o O) (indexed by row in MODE 0, by column in MODE 1) are written as
 // K-major SWIZZLE_128B A tiles; then  MODE 0: acc += dS Y1 (= dS K);  MODE 1: accV += P^T Y2 (= P^T dO),
 // accK += dS^T Y1 (= dS^T Q) with the streamed tiles read MN-major, exactly like V in the forward kernel.
 // MODE 0 also computes delta (it owns dO and reads O) and stores it for the MODE 1 launch that follows it in stream order.
@@ -439,7 +333,6 @@ struct AttnBwdParams {
     int nq;                  // query count (lse / delta row pitch)
     void* dS;                // MODE 0, optional: dS = P o (dP - delta) * scale exported as [images*heads][nq][ldds] (16-bit)
     long long ldds;
-    unsigned idesc_t, idesc_acc;
 };
 
 template <int DBOX, int MODE>
@@ -449,34 +342,16 @@ struct AttnBwdCfg {
     static constexpr int kABytes = kBQ * 128;               // one A tile (128 rows x 64 block items)
     static constexpr int kNumA = MODE == 0 ? 1 : 2;
     static constexpr int kNumAcc = MODE == 0 ? 1 : 2;
-    static constexpr int kSmemBytes = 2 * kXBytes + 2 * 2 * kYBytes + kNumA * kABytes + 1024 + 256 + 1024;
-    static constexpr int kTmemNeed = 128 + kNumAcc * DBOX * 64;
-    static constexpr int kTmemCols = kTmemNeed <= 256 ? 256 : 512;
-    static constexpr int kMinBlocks = (kTmemCols <= 256 && kSmemBytes <= 110 * 1024) ? 2 : 1;
+    static constexpr int kSmemBytes = 2 * kXBytes + 2 * 2 * kYBytes + kNumA * kABytes + 1024 + 256;
 };
 
-__device__ __forceinline__ uint4 store_a16(uint32_t tile, int r, int key8, const float (&e)[8], bool bf16) {
-    uint4 pk;
-    if (bf16) {
-        __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(e[2 * i], e[2 * i + 1]);
-    } else {
-        __half2* h = reinterpret_cast<__half2*>(&pk);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(e[2 * i], e[2 * i + 1]);
-    }
-    const uint32_t dst = tile + r * 128 + ((key8 ^ (r & 7)) << 4);
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk.x), "r"(pk.y), "r"(pk.z), "r"(pk.w) : "memory");
-    return pk;
-}
-
 template <int DBOX, int MODE>
-__global__ void __launch_bounds__(kAttnThreads, AttnBwdCfg<DBOX, MODE>::kMinBlocks)
+__global__ void __launch_bounds__(kAttnThreads, 1)
 cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                         const __grid_constant__ CUtensorMap tmY1, const __grid_constant__ CUtensorMap tmY2,
                         const __grid_constant__ AttnBwdParams p) {
     using Cfg = AttnBwdCfg<DBOX, MODE>;
+    constexpr int NO = DBOX * 64;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t sX1 = base, sX2 = base + Cfg::kXBytes;
@@ -486,12 +361,7 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
     const uint32_t bar_x = bars;
     auto bar_y_full = [&](int s) { return bars + 8u * (1 + s); };
     auto bar_y_empty = [&](int s) { return bars + 8u * (3 + s); };
-    const uint32_t bar_t_full = bars + 8u * 5;
-    const uint32_t bar_t_empty = bars + 8u * 6;
-    const uint32_t bar_a_full = bars + 8u * 7;
-    const uint32_t bar_a_done = bars + 8u * 8;
-    const uint32_t tmem_slot = bars + 8u * 9;
-    float* s_stat = reinterpret_cast<float*>(smem_raw + (bars + 256 - smem_u32(smem_raw)));    // [2 buffers][2][64] (MODE 1)
+    __shared__ float2 s_stat[2][kBKV];         // MODE 1: (lse*log2e, delta*scale) of the streamed queries, per warpgroup
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int x0 = blockIdx.x * kBQ;
@@ -504,28 +374,17 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
     }
     const int nit = max(0, jend - jbeg);
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmX1); tma_prefetch_desc(&tmX2); tma_prefetch_desc(&tmY1); tma_prefetch_desc(&tmY2);
         mbar_init(bar_x, 1);
-        for (int s = 0; s < 2; ++s) { mbar_init(bar_y_full(s), 1); mbar_init(bar_y_empty(s), 1); }
-        mbar_init(bar_t_full, 1);
-        mbar_init(bar_t_empty, 128);
-        mbar_init(bar_a_full, 128);
-        mbar_init(bar_a_done, 1);
+        for (int s = 0; s < 2; ++s) { mbar_init(bar_y_full(s), 1); mbar_init(bar_y_empty(s), kAttnConsumers); }
         mbar_fence_init();
         fence_proxy_async_smem();
     }
-    if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-    __syncwarp();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem) : "r"(tmem_slot));
-    const uint32_t tT1 = tmem, tT2 = tmem + 64, tAcc0 = tmem + 128, tAcc1 = tmem + 128 + DBOX * 64;
     pdl_sync();
 
-    if (warp == 0) {
+    if (warp == kAttnConsumers / 32) {
         if (lane == 0) {
             mbar_arrive_expect_tx(bar_x, 2 * Cfg::kXBytes);
 #pragma unroll
@@ -545,76 +404,35 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const int ks = p.dpad16 / 16;
-            auto issue_T = [&](int it) {
-                const int s = it & 1;
-                mbar_wait(bar_y_full(s), (it >> 1) & 1);
-                mbar_wait(bar_t_empty, (it & 1) ^ 1u);
-                tc_fence_after();
-                const uint32_t y1 = sY + s * 2 * Cfg::kYBytes, y2 = y1 + Cfg::kYBytes;
-                for (int k = 0; k < ks; ++k) {
-                    const uint32_t offx = (k >> 2) * (kBQ * 128) + (k & 3) * 32;
-                    const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-                    umma_f16(tT1, umma_smem_desc_sw128(sX1 + offx, 16, 1024), umma_smem_desc_sw128(y1 + offy, 16, 1024),
-                             p.idesc_t, k > 0 ? 1u : 0u);
-                }
-                for (int k = 0; k < ks; ++k) {
-                    const uint32_t offx = (k >> 2) * (kBQ * 128) + (k & 3) * 32;
-                    const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-                    umma_f16(tT2, umma_smem_desc_sw128(sX2 + offx, 16, 1024), umma_smem_desc_sw128(y2 + offy, 16, 1024),
-                             p.idesc_t, k > 0 ? 1u : 0u);
-                }
-                umma_commit(bar_t_full);
-            };
-            mbar_wait(bar_x, 0);
-            if (nit > 0) issue_T(0);
-            for (int it = 0; it < nit; ++it) {
-                if (it + 1 < nit) issue_T(it + 1);
-                const int s = it & 1;
-                mbar_wait(bar_a_full, it & 1);
-                tc_fence_after();
-                const uint32_t y1 = sY + s * 2 * Cfg::kYBytes, y2 = y1 + Cfg::kYBytes;
-                for (int k = 0; k < kBKV / 16; ++k) {
-                    const uint64_t a0 = umma_smem_desc_sw128(sA + k * 32, 16, 1024);
-                    if (MODE == 0) {
-                        umma_f16(tAcc0, a0, umma_smem_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), p.idesc_acc, (it > 0 || k > 0) ? 1u : 0u);
-                    } else {
-                        const uint64_t a1 = umma_smem_desc_sw128(sA + Cfg::kABytes + k * 32, 16, 1024);
-                        umma_f16(tAcc0, a0, umma_smem_desc_sw128(y2 + k * 2048, kBKV * 128, 1024), p.idesc_acc, (it > 0 || k > 0) ? 1u : 0u);
-                        umma_f16(tAcc1, a1, umma_smem_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), p.idesc_acc, (it > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                umma_commit(bar_y_empty(s));
-                umma_commit(bar_a_done);
-            }
-        }
-    } else {
-        // ====================== one thread per stationary row ======================
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        const int xrow = x0 + r;
-        const bool row_ok = xrow < p.n_stat;
-        const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
-        const int et = threadIdx.x - 64;
-        const long long stat_base = (static_cast<long long>(img) * p.heads + head) * p.nq;
-        const float kLog2e = 1.4426950408889634f;
-        float lse_r = 0.f, delta_r = 0.f;          // MODE 0: this query row's statistics
-        float nlse = 0.f, ndelta = 0.f;            // MODE 1: prefetched column statistics of the next block (threads et < 64)
-        if (MODE == 0) {
-            if (row_ok) {
-                lse_r = p.lse[stat_base + xrow] * kLog2e;
+        return;
+    }
+
+    // ====================== consumers: 64 stationary rows per warpgroup ======================
+    const int wg = warp >> 2;
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
+    const int cq = 2 * (lane & 3);
+    const int et = threadIdx.x & 127;                          // thread index inside the warpgroup
+    const bool bf16 = p.is_bf16 != 0;
+    const uint32_t xoff = static_cast<uint32_t>(wg) * 8192u;
+    const long long stat_base = (static_cast<long long>(img) * p.heads + head) * p.nq;
+    const float kLog2e = 1.4426950408889634f;
+    float lse_r[2] = {0.f, 0.f}, delta_r[2] = {0.f, 0.f};     // MODE 0: this thread's query rows' statistics
+    if (MODE == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int xrow = x0 + rl + 8 * h;
+            float acc = 0.f;
+            if (xrow < p.n_stat) {
+                lse_r[h] = p.lse[stat_base + xrow] * kLog2e;
                 const uint16_t* orow = reinterpret_cast<const uint16_t*>(p.O) + (static_cast<long long>(img) * p.n_stat + xrow) * p.ldo + static_cast<long long>(head) * p.d;
                 const uint16_t* grow = reinterpret_cast<const uint16_t*>(p.dO) + (static_cast<long long>(img) * p.n_stat + xrow) * p.lddo + static_cast<long long>(head) * p.d;
-                float acc = 0.f;
-                for (int c = 0; c < p.d; c += 8) {
+                for (int c = (lane & 3) * 8; c < p.d; c += 32) {       // the four lanes of a row split its 8-column groups
                     const uint4 a = *reinterpret_cast<const uint4*>(orow + c), b = *reinterpret_cast<const uint4*>(grow + c);
                     const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
                     for (int i = 0; i < 4; ++i) {
                         float2 fa, fb;
-                        if (p.is_bf16) {
+                        if (bf16) {
                             fa = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[i]));
                             fb = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&bw[i]));
                         } else {
@@ -624,135 +442,159 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
                         acc += fa.x * fb.x + fa.y * fb.y;
                     }
                 }
-                delta_r = acc * p.scale;            // used as fma(T2, scale, -delta*scale)
-                p.delta[stat_base + xrow] = acc;
             }
-        } else if (et < 64 && nit > 0) {
-            const int qc = jbeg * kBKV + et;
-            if (qc < p.n_stream) { nlse = p.lse[stat_base + qc] * kLog2e; ndelta = p.delta[stat_base + qc] * p.scale; }
-        }
-        for (int it = 0; it < nit; ++it) {
-            const int j = jbeg + it;
-            const int cbase = j * kBKV;
-            float2* st_ld = reinterpret_cast<float2*>(s_stat) + (it & 1) * 64;     // (lse*log2e, delta*scale) per streamed query
-            if (MODE == 1) {
-                if (et < 64) st_ld[et] = make_float2(nlse, ndelta);
-                asm volatile("bar.sync 3, 128;" ::: "memory");
-                if (et < 64 && it + 1 < nit) {
-                    const int qc = (j + 1) * kBKV + et;
-                    nlse = 0.f; ndelta = 0.f;
-                    if (qc < p.n_stream) { nlse = p.lse[stat_base + qc] * kLog2e; ndelta = p.delta[stat_base + qc] * p.scale; }
-                }
-            }
-            // valid streamed items of this block for this row
-            int cvalid = min(kBKV, p.n_stream - cbase);      // columns past the end of the streamed operand
-            int cfirst = 0;
-            if (p.causal) {
-                if (MODE == 0) cvalid = min(cvalid, xrow - cbase + 1);      // keys <= this query
-                else cfirst = max(0, xrow - cbase);                         // queries >= this key
-            }
-            if (!row_ok && MODE == 0) cvalid = 0;
-            mbar_wait(bar_t_full, it & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                uint32_t t1[32], t2[32];
-                tmem_ld_32x32(tT1 + lane_off + half * 32, t1);
-                tmem_ld_32x32(tT2 + lane_off + half * 32, t2);
-                tmem_ld_wait();
-                if (half == 1) {
-                    tc_fence_before();
-                    mbar_arrive(bar_t_empty);           // T1/T2 may be overwritten by the next block's MMAs
-                } else if (it > 0) {
-                    mbar_wait(bar_a_done, (it - 1) & 1);    // the previous block's accumulation MMAs have read the A tiles
-                    tc_fence_after();
-                }
-                // P = ex2(fma(T1, scale*log2e, -lse*log2e)); dS = P * fma(T2, scale, -delta*scale).  Unmasked blocks (all
-                // but the ragged tail / the causal diagonal) skip the per-element predicates.
-                const bool masked = cvalid < kBKV || cfirst > 0;
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    float pe[8], ds[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int c = half * 32 + g * 8 + i;
-                        float l2, dl;
-                        if (MODE == 0) { l2 = lse_r; dl = delta_r; }
-                        else { const float2 sd = st_ld[c]; l2 = sd.x; dl = sd.y; }
-                        float pv = fast_exp2(fmaf(__uint_as_float(t1[g * 8 + i]), p.scale_log2e, -l2));
-                        if (masked) pv = (c < cvalid && c >= cfirst) ? pv : 0.f;
-                        pe[i] = pv;
-                        ds[i] = pv * fmaf(__uint_as_float(t2[g * 8 + i]), p.scale, -dl);
-                    }
-                    const int key8 = half * 4 + g;
-                    if (MODE == 0) {
-                        const uint4 pk = store_a16(sA, r, key8, ds, p.is_bf16 != 0);
-                        if (p.dS && row_ok && cbase + key8 * 8 < p.ldds)
-                            *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(p.dS) + (stat_base + xrow) * p.ldds + cbase + key8 * 8) = pk;
-                    } else {
-                        store_a16(sA, r, key8, pe, p.is_bf16 != 0);
-                        store_a16(sA + Cfg::kABytes, r, key8, ds, p.is_bf16 != 0);
-                    }
-                }
-            }
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(bar_a_full);
-        }
-        if (MODE == 0 && p.dS && row_ok) {
-            // causal: key blocks past this tile's last query were never visited -- their dS is zero
-            const int nblk_all = (p.n_stream + kBKV - 1) / kBKV;
-            uint16_t* dsrow = reinterpret_cast<uint16_t*>(p.dS) + (stat_base + xrow) * p.ldds;
-            for (int j = jend; j < nblk_all; ++j)
-                for (int key8 = 0; key8 < 8; ++key8)
-                    if (j * kBKV + key8 * 8 < p.ldds) *reinterpret_cast<uint4*>(dsrow + j * kBKV + key8 * 8) = make_uint4(0u, 0u, 0u, 0u);
-        }
-        // ---- epilogue: accumulators -> HBM ----
-        if (nit > 0) mbar_wait(bar_a_done, (nit - 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int a = 0; a < Cfg::kNumAcc; ++a) {
-            const uint32_t tacc = a == 0 ? tAcc0 : tAcc1;
-            uint16_t* outp = reinterpret_cast<uint16_t*>(a == 0 ? p.out1 : p.out2);
-            if (outp == nullptr) continue;
-            const long long ldout = a == 0 ? p.ld1 : p.ld2;
-            for (int c = 0; c * 32 < DBOX * 64; ++c) {
-                if (c * 32 >= p.d) break;
-                uint32_t o[32];
-                if (nit > 0) {
-                    tmem_ld_32x32(tacc + lane_off + c * 32, o);
-                    tmem_ld_wait();
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o[i] = 0u;
-                }
-                if (row_ok) {
-                    const long long orow = (static_cast<long long>(img) * p.n_stat + xrow) * ldout + static_cast<long long>(head) * p.d;
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int col = c * 32 + g * 8;
-                        if (col < p.d) {
-                            uint4 pk;
-                            if (p.is_bf16) {
-                                __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&pk);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(__uint_as_float(o[g * 8 + 2 * i]), __uint_as_float(o[g * 8 + 2 * i + 1]));
-                            } else {
-                                __half2* h = reinterpret_cast<__half2*>(&pk);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(__uint_as_float(o[g * 8 + 2 * i]), __uint_as_float(o[g * 8 + 2 * i + 1]));
-                            }
-                            *reinterpret_cast<uint4*>(outp + orow + col) = pk;
-                        }
-                    }
-                }
-            }
+            acc = quad_sum(acc);
+            delta_r[h] = acc * p.scale;            // used as fma(T2, scale, -delta*scale)
+            if (xrow < p.n_stat && (lane & 3) == 0) p.delta[stat_base + xrow] = acc;
         }
     }
-    __syncwarp();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem);
+    // acc1: MODE 1 only.  Neither is initialised: the first block's MMAs overwrite them (scale_d = 0), and an accumulator
+    // written by ordinary instructions would make ptxas serialise every wgmma of the loop.
+    float acc0[NO / 2], acc1[NO / 2];
+    const int ks = p.dpad16 / 16;
+    mbar_wait(bar_x, 0);
+    for (int it = 0; it < nit; ++it) {
+        const int j = jbeg + it;
+        const int cbase = j * kBKV;
+        const int s = it & 1;
+        if (MODE == 1 && et < kBKV) {
+            const int qc = cbase + et;
+            s_stat[wg][et] = qc < p.n_stream ? make_float2(p.lse[stat_base + qc] * kLog2e, p.delta[stat_base + qc] * p.scale)
+                                             : make_float2(0.f, 0.f);
+        }
+        // the statistics are in place, and every thread of this warpgroup is past the previous block's accumulation MMAs
+        // (the A tiles below may be overwritten)
+        named_bar(1 + wg, 128);
+        mbar_wait(bar_y_full(s), (it >> 1) & 1);
+        const uint32_t y1 = sY + s * 2 * Cfg::kYBytes, y2 = y1 + Cfg::kYBytes;
+        // valid streamed items of this block for each of this thread's rows
+        int cvalid[2], cfirst[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int xrow = x0 + rl + 8 * h;
+            cvalid[h] = min(kBKV, p.n_stream - cbase);      // columns past the end of the streamed operand
+            cfirst[h] = 0;
+            if (p.causal) {
+                if (MODE == 0) cvalid[h] = min(cvalid[h], xrow - cbase + 1);      // keys <= this query
+                else cfirst[h] = max(0, xrow - cbase);                            // queries >= this key
+            }
+            if (MODE == 0 && xrow >= p.n_stat) cvalid[h] = 0;
+        }
+        float t[32];
+        wgmma_fence();
+        for (int k = 0; k < ks; ++k) {
+            const uint32_t offx = (k >> 2) * (kBQ * 128) + xoff + (k & 3) * 32;
+            const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
+            wgmma_any<64, 0, 0>(bf16, t, gmma_desc_sw128(sX1 + offx, 16, 1024), gmma_desc_sw128(y1 + offy, 16, 1024), k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(t);
+        // P = ex2(fma(T1, scale*log2e, -lse*log2e)), zero outside the valid block items
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int col = jj * 8 + cq + c;
+                    const float l2 = MODE == 0 ? lse_r[h] : s_stat[wg][col].x;
+                    const float pv = fast_exp2(fmaf(t[4 * jj + 2 * h + c], p.scale_log2e, -l2));
+                    t[4 * jj + 2 * h + c] = (col < cvalid[h] && col >= cfirst[h]) ? pv : 0.f;
+                }
+        if (MODE == 1) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) st_a_pair(sA, rl + 8 * h, jj * 8 + cq, pack2(t[4 * jj + 2 * h], t[4 * jj + 2 * h + 1], bf16));
+        }
+        float t2[32];
+        wgmma_fence();
+        for (int k = 0; k < ks; ++k) {
+            const uint32_t offx = (k >> 2) * (kBQ * 128) + xoff + (k & 3) * 32;
+            const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
+            wgmma_any<64, 0, 0>(bf16, t2, gmma_desc_sw128(sX2 + offx, 16, 1024), gmma_desc_sw128(y2 + offy, 16, 1024), k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(t2);
+        // dS = P * fma(T2, scale, -delta*scale)
+        const uint32_t ds_tile = MODE == 0 ? sA : sA + Cfg::kABytes;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int xrow = x0 + rl + 8 * h;
+            uint32_t* dsrow = (MODE == 0 && p.dS && xrow < p.n_stat)
+                                  ? reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.dS) + (stat_base + xrow) * p.ldds + cbase + cq)
+                                  : nullptr;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                float ds[2];
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const float dl = MODE == 0 ? delta_r[h] : s_stat[wg][jj * 8 + cq + c].y;
+                    ds[c] = t[4 * jj + 2 * h + c] * fmaf(t2[4 * jj + 2 * h + c], p.scale, -dl);
+                }
+                const uint32_t v = pack2(ds[0], ds[1], bf16);
+                st_a_pair(ds_tile, rl + 8 * h, jj * 8 + cq, v);
+                if (dsrow && cbase + jj * 8 < p.ldds) dsrow[jj * 4] = v;
+            }
+        }
+        fence_proxy_async_smem();
+        named_bar(1 + wg, 128);                    // this warpgroup's 64 rows of the A tiles are complete
+        wgmma_fence_regs(acc0);
+        if constexpr (MODE == 1) wgmma_fence_regs(acc1);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBKV / 16; ++k) {
+            const uint64_t a0 = gmma_desc_sw128(sA + xoff + k * 32, 16, 1024);
+            const uint32_t acc_in = (it > 0 || k > 0) ? 1u : 0u;
+            if constexpr (MODE == 0) {
+                wgmma_any<NO, 0, 1>(bf16, acc0, a0, gmma_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), acc_in);
+            } else {
+                const uint64_t a1 = gmma_desc_sw128(sA + Cfg::kABytes + xoff + k * 32, 16, 1024);
+                wgmma_any<NO, 0, 1>(bf16, acc0, a0, gmma_desc_sw128(y2 + k * 2048, kBKV * 128, 1024), acc_in);
+                wgmma_any<NO, 0, 1>(bf16, acc1, a1, gmma_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), acc_in);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc0);
+        if constexpr (MODE == 1) wgmma_fence_regs(acc1);
+        mbar_arrive(bar_y_empty(s));
+    }
+    if (MODE == 0 && p.dS) {
+        // causal: key blocks past this tile's last query were never visited -- their dS is zero
+        const int nblk_all = (p.n_stream + kBKV - 1) / kBKV;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int xrow = x0 + rl + 8 * h;
+            if (xrow >= p.n_stat) continue;
+            uint16_t* dsrow = reinterpret_cast<uint16_t*>(p.dS) + (stat_base + xrow) * p.ldds;
+            for (int jb = jend; jb < nblk_all; ++jb)
+                for (int key8 = lane & 3; key8 < 8; key8 += 4)
+                    if (jb * kBKV + key8 * 8 < p.ldds) *reinterpret_cast<uint4*>(dsrow + jb * kBKV + key8 * 8) = make_uint4(0u, 0u, 0u, 0u);
+        }
+    }
+    // ---- epilogue: accumulators -> HBM ----
+    auto store_acc = [&](const float (&acc)[NO / 2], void* out, long long ldout) {
+        uint16_t* outp = reinterpret_cast<uint16_t*>(out);
+        if (outp == nullptr) return;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int xrow = x0 + rl + 8 * h;
+            if (xrow >= p.n_stat) continue;
+            uint16_t* orow = outp + (static_cast<long long>(img) * p.n_stat + xrow) * ldout + static_cast<long long>(head) * p.d;
+#pragma unroll
+            for (int jj = 0; jj < NO / 8; ++jj) {
+                const int col = jj * 8 + cq;
+                if (col < p.d)                                 // no streamed block (causal corner): the result is zero
+                    *reinterpret_cast<uint32_t*>(orow + col) =
+                        nit > 0 ? pack2(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1], bf16) : 0u;
+            }
+        }
+    };
+    store_acc(acc0, p.out1, p.ld1);
+    if constexpr (MODE == 1) store_acc(acc1, p.out2, p.ld2);
 }
 
 template <int DBOX, int MODE>
@@ -783,9 +625,6 @@ static int attn_tmap(CUtensorMap* out, int dtype, const void* ptr, long long ld,
 
 using namespace cb;
 
-static unsigned long long* g_attn_dbg = nullptr;
-// profiling hook (not part of the public header): device buffer of 8 x uint64 per CTA, or NULL to disable
-extern "C" void cb_debug_attention_timeline(void* buf) { g_attn_dbg = reinterpret_cast<unsigned long long*>(buf); }
 
 extern "C" int cb_attention_fwd(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv,
                                 void* O, long long ldo, float* lse, void* P, long long ldp, int dtype, int images,
@@ -805,11 +644,7 @@ extern "C" int cb_attention_fwd(const void* Q, long long ldq, const void* K, lon
     p.O = O; p.o_dtype = dtype; p.ldo = ldo; p.lse = lse;
     p.P = P; p.ldp = ldp; p.p_is_bf16 = dtype == CB_BF16;
     p.two_pass = P != nullptr ? 1 : 0;
-    p.dbg = g_attn_dbg;
     if (P) CB_REQUIRE(ldp >= nk && ldp % 8 == 0 && (reinterpret_cast<uintptr_t>(P) & 15u) == 0, CB_ERR_ALIGN, "attention_fwd: P row pitch must be a multiple of 8 elements >= nk");
-    // S = Q K^T : M=128, N=128 keys, both K-major.  O = P V : M=128, N=dpad16, A K-major, B (V) MN-major.
-    p.idesc_s = umma_idesc_f16(128, kBKV, dtype == CB_BF16, false, false);
-    p.idesc_o = umma_idesc_f16(128, p.dboxes * 64, dtype == CB_BF16, false, true);   // N = whole 64-col chunks (zero-filled past d)
     CUtensorMap tq, tk, tv;
     uint32_t estr[4] = {1, 1, 1, 1};
     uint32_t box[4] = {64, kBQ, 1, 1};
@@ -857,8 +692,6 @@ static int attention_bwd_impl(const void* Q, long long ldq, const void* K, long 
     p.causal = causal; p.scale = scale; p.scale_log2e = scale * 1.4426950408889634f;
     p.lse = lse; p.delta = delta; p.O = O; p.dO = dO; p.ldo = ldo; p.lddo = lddo;
     p.is_bf16 = dtype == CB_BF16; p.nq = nq;
-    p.idesc_t = umma_idesc_f16(128, kBKV, dtype == CB_BF16, false, false);
-    p.idesc_acc = umma_idesc_f16(128, p.dboxes * 64, dtype == CB_BF16, false, true);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CUtensorMap x1, x2, y1, y2;
     int rc = 0;

@@ -1,9 +1,9 @@
-// celebbasis_b200 — shared device/host helpers for the sm_100a kernels.
+// celebbasis_b200 — shared device/host helpers for the sm_90a kernels.
 //
-// Everything here is hand-written PTX wrappers for the Blackwell execution model
-// (mbarrier, TMA bulk-tensor loads, tcgen05 MMA / TMEM) plus the error plumbing of the
-// C-ABI.  No CUTLASS/CuTe types are used; bit layouts of the UMMA descriptors follow the
-// PTX ISA tables (cross-checked against cute/arch/mma_sm100_desc.hpp field comments).
+// Everything here is hand-written PTX wrappers for the Hopper execution model
+// (mbarrier, TMA bulk-tensor loads, wgmma, thread-block clusters) plus the error plumbing of the
+// C-ABI.  No CUTLASS/CuTe types are used; bit layouts of the wgmma descriptors follow the
+// PTX ISA tables.
 #pragma once
 
 #include <cuda.h>
@@ -13,6 +13,7 @@
 #include <stdint.h>
 
 #include "../../include/celebbasis_b200.h"
+#include "cb_wgmma.cuh"
 
 namespace cb {
 
@@ -199,69 +200,26 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint
                  : "memory");
 }
 
-// ---- tcgen05 / TMEM -------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// ---- wgmma (warpgroup MMA, fp32 accumulators in registers) -----------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+// runtime fp16 / bf16 selection of the same wgmma shape
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_any(bool bf16, float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+    if (bf16) Wgmma<N, true, TA, TB>::mma(d, a, b, scale_d);
+    else Wgmma<N, false, TA, TB>::mma(d, a, b, scale_d);
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_result_addr) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_result_addr),
-                 "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread for the CTA.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (one row per thread).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-          "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-          "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// TMEM -> registers: this warp's 32 lanes x 8 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// named barrier over `n` threads (n a multiple of 32); ids 0..15
+__device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
-// ---- CTA pair (cta_group::2): two CTAs of a cluster on one TPC share one 256-row MMA -------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -269,44 +227,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_result_addr) {      // one warp in EACH CTA of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_result_addr), "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem of both CTAs, 256 rows] (+)= A[128 rows in each CTA's smem] * B[N/2 columns in each CTA's smem]; leader CTA only.
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in BOTH CTAs once the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-// TMA load into THIS CTA's shared memory whose transaction bytes are credited to the LEADER CTA's mbarrier (peer bit cleared)
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2,
-                                                 int c3) {
-    const uint32_t leader_bar = bar & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-        "%5, %6}], [%2];" ::"r"(dst),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
 }
 
 // 32 bytes (8 floats) into the shared memory of CTA `cta` of the cluster at the offset `addr` has in this CTA
@@ -340,38 +260,17 @@ __device__ __forceinline__ float4 ld_shared_f32x4(uint32_t addr) {
     return v;
 }
 
-// arrive (release, cluster scope) on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-    asm volatile(
-        "{\n"
-        ".reg .b32 ra;\n"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
-        "}\n" ::"r"(bar),
-        "r"(cta)
-        : "memory");
-}
-
-// ---- UMMA descriptors -------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit): [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 |
-// [46,48) version=1 | [49,52) base offset | [61,64) layout (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// ---- wgmma shared-memory matrix descriptor (SWIZZLE_128B) ---------------------------------------------------
+// [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset (0: 1 KiB aligned atoms) | [62,64) layout (1 = 128B
+// swizzle).  K-major: SBO = 1024 (8-row groups), LBO unused; a 16-element k step adds 32 bytes to the start address.
+// MN-major: LBO = bytes between 64-element MN blocks, SBO = 1024 (8 k rows); a 16-row k step adds 2048 bytes.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
-}
-// Instruction descriptor for kind::f16 (fp16/bf16 in, fp32 accumulate):
-// [4,6) c_format (1=f32) | [7,10) a_format | [10,13) b_format (0=f16,1=bf16) | bit15 a_major |
-// bit16 b_major (0=K-major,1=MN-major) | [17,23) N>>3 | [24,29) M>>4.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, bool bf16, bool a_mn, bool b_mn) {
-    return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((a_mn ? 1u : 0u) << 15) |
-           ((b_mn ? 1u : 0u) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-           (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 // ---- small math ---------------------------------------------------------------------------------------

@@ -67,7 +67,8 @@ __device__ __forceinline__ void jitter_pixel(float& r, float& g, float& b, const
 }
 
 // iparams [B][5] = {flip, order0..3}; fparams [B][4] = {brightness, contrast, saturation, hue}
-// pass 1: sum over the image of gray(ops before the contrast op) -> gsum[b] (double)
+// pass 1: sum over the image of gray(ops before the contrast op) -> gsum[b] (double); one CTA per image, so the sum is
+// taken in a fixed order
 __global__ void jitter_mean_kernel(const uint8_t* __restrict__ src, const int* __restrict__ iparams,
                                    const float* __restrict__ fparams, double* __restrict__ gsum, int HW) {
     const int b = blockIdx.y;
@@ -93,7 +94,7 @@ __global__ void jitter_mean_kernel(const uint8_t* __restrict__ src, const int* _
     if (warp == 0) {
         float v = lane < (blockDim.x >> 5) ? s_part[lane] : 0.f;
         v = warp_sum(v);
-        if (lane == 0 && n_before >= 0) atomicAdd(gsum + b, (double)v);
+        if (lane == 0 && n_before >= 0) gsum[b] = (double)v;
     }
 }
 
@@ -168,7 +169,7 @@ extern "C" int cb_face_augment(const unsigned char* src_u8, const int* iparams, 
     CB_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * B, st));
     const int HW = H * W;
     dim3 grid((unsigned)std::min(ceil_div(HW, 256 * 4), 4 * device_sm_count()), (unsigned)B);
-    jitter_mean_kernel<<<grid, 256, 0, st>>>(src_u8, iparams, fparams, ws, HW);
+    jitter_mean_kernel<<<dim3(1, (unsigned)B), 1024, 0, st>>>(src_u8, iparams, fparams, ws, HW);
     face_augment_kernel<<<grid, 256, 0, st>>>(src_u8, iparams, fparams, ws, out, H, W, c_total, c_off);
     CB_CUDA(cudaGetLastError());
     count_launches(2);

@@ -172,14 +172,17 @@ __global__ void embed_inject_fwd_kernel(const float* __restrict__ tok, const flo
     const float* src = m >= 0 ? tok + ((size_t)b * T + m) * D : z + (size_t)(-(m + 1)) * D;
     for (int c = threadIdx.x; c < D; c += blockDim.x) out[(size_t)row * D + c] = src[c] + pos[(size_t)i * D + c];
 }
+// one CTA per z row: the token rows that received it are summed in row order (bit-identical from run to run)
 __global__ void embed_inject_bwd_kernel(const float* __restrict__ dout, const int* __restrict__ map,
-                                        float* __restrict__ dz, int D) {
+                                        float* __restrict__ dz, int rows, int D) {
     pdl_sync();
-    const int row = blockIdx.x;
-    const int m = map[row];
-    if (m >= 0) return;
-    float* dst = dz + (size_t)(-(m + 1)) * D;
-    for (int c = threadIdx.x; c < D; c += blockDim.x) atomicAdd(dst + c, dout[(size_t)row * D + c]);
+    const int zr = blockIdx.x;
+    for (int c = threadIdx.x; c < D; c += blockDim.x) {
+        float acc = 0.f;
+        for (int row = 0; row < rows; ++row)
+            if (map[row] == -(zr + 1)) acc += dout[(size_t)row * D + c];
+        dz[(size_t)zr * D + c] = acc;
+    }
 }
 
 __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
@@ -366,8 +369,7 @@ extern "C" int cb_embed_inject_bwd(const float* dout, const int* map, float* dz,
                                    void* stream) {
     CB_REQUIRE(B > 0 && T > 0 && D > 0 && n_z_rows > 0, CB_ERR_ARG, "embed_inject_bwd: bad shape");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    CB_CUDA(cudaMemsetAsync(dz, 0, sizeof(float) * (size_t)n_z_rows * D, st));
-CB_LAUNCH((embed_inject_bwd_kernel), B * T, 256, 0, st, dout, map, dz, D);
+    CB_LAUNCH((embed_inject_bwd_kernel), n_z_rows, 256, 0, st, dout, map, dz, B * T, D);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
     return 0;

@@ -1,14 +1,12 @@
-// cb_gemm — tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// cb_gemm — wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
 // One CTA computes one 128 x BN output tile:
-//   warp 0      : TMA producer (cp.async.bulk.tensor, SWIZZLE_128B boxes, mbarrier complete_tx)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (fp32 accumulator in TMEM)
-//   warps 2..5  : epilogue (tcgen05.ld 32x32b -> registers -> alpha/bias/act/residual -> HBM)
+//   thread 0         : TMA producer (cp.async.bulk.tensor, SWIZZLE_128B boxes, mbarrier complete_tx)
+//   warpgroups 1, 2  : wgmma.mma_async on 64 rows each, fp32 accumulators in registers
+//   warpgroup 0      : epilogue (staged accumulator rows -> alpha/bias/act/residual -> HBM)
 // Convolutions never materialise im2col: each (tap, 64-channel) k-iteration loads a SHIFTED
 // [box_i][box_h][box_w][64ch] box of the NHWC image straight into the K-major A tile; padding is
 // the TMA out-of-bounds zero fill, stride-2 is the tensor-map traversal stride.
-// Two CTAs are resident per SM (3-stage ring each) so one tile's epilogue overlaps the
-// other's MMA main loop.
 #include <algorithm>
 #include <stdarg.h>
 #include <stdio.h>
@@ -21,7 +19,7 @@ namespace cb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;
 
 struct GemmParams {
     int M, N, K;
@@ -47,7 +45,7 @@ struct GemmParams {
     int d_transposed;
     int vec_ok;
     int force_stages;  // 0 auto / 3 / 6 (cb_gemm_desc.stages)
-    int vec32_ok;     // D (and R) rows are 32-byte aligned: 256-bit LDG/STG (sm_100) in the epilogue
+    int vec32_ok;     // D (and R) rows are 32-byte aligned: one 32-byte sector per lane and chunk in the epilogue
     const float* bias;
     int bias_row_div;
     long long ldbias;
@@ -56,10 +54,10 @@ struct GemmParams {
     long long ldr, r_bs, r_bs2;
     float alpha;
     int act;
-    unsigned idesc;
+    int bf16;                 // operands are bf16 (else fp16)
     unsigned a_bytes, b_bytes;
-    // split-K: the k-iterations of one output tile are spread over `splits` CTAs which red.add their fp32 partials
-    // into the tile's accumulator in `ws`; the last CTA to arrive (per-tile counter) runs the epilogue.
+    // split-K: the k-iterations of one output tile are spread over `splits` CTAs which store their fp32 partials into
+    // the tile's slices of `ws`; the last CTA to arrive (per-tile counter) sums them in slice order and runs the epilogue.
     int splits, kiters_per_split;
     float* ws;
     unsigned* counters;
@@ -76,6 +74,7 @@ struct TileCfg {
     static constexpr int kBBytes = BN * BK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
+    static_assert(kStages * kStageBytes >= BM * (BN + 4) * 4, "the accumulator tile is staged in the TMA ring");
 };
 
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -191,15 +190,14 @@ __device__ __forceinline__ void store8_any(void* base, int dtype, long long idx,
 // needed (the loads are in flight while the MMAs / the previous chunk's stores run; D may alias R, so the compiler could
 // never hoist them itself).
 struct ResidualChunk { uint4 v[8]; };
+// one 32-byte sector as two 16-byte accesses (sm_90 has no 256-bit global load / store)
 __device__ __forceinline__ void ldg256(const void* ptr, uint4& a, uint4& b) {
-    asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(ptr));
+    a = reinterpret_cast<const uint4*>(ptr)[0];
+    b = reinterpret_cast<const uint4*>(ptr)[1];
 }
 __device__ __forceinline__ void stg256(void* ptr, const uint4& a, const uint4& b) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(a.x), "r"(a.y), "r"(a.z),
-                 "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
+    reinterpret_cast<uint4*>(ptr)[0] = a;
+    reinterpret_cast<uint4*>(ptr)[1] = b;
 }
 __device__ __forceinline__ void residual_prefetch(const GemmParams& p, long long ridx, ResidualChunk& rc) {
     if (p.r_dtype == CB_F32) {
@@ -425,38 +423,35 @@ __device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const floa
     }
 }
 
-// ---- split-K hand-off (epilogue warps, 128 threads; shared by the single-CTA and the CTA-pair kernels): every CTA adds its
-//      fp32 partial tile into one L2-resident accumulator tile with vector reductions (red.global.add.v4.f32, spread over
-//      all L2 slices); the last CTA to arrive (per-tile counter) reads the sum, runs the epilogue and re-zeroes tile +
-//      counter for the next launch.  `tmem_done()` runs once this thread's last TMEM read has completed.
-//      accumulator-tile layout (p.ws_tr): float4 group g (= 4 columns) of row r lives at ((g * BM) + r) * 4 floats, so the
-//      32 lanes of a warp (32 consecutive rows) touch 512 contiguous bytes per reduction / load / store -- four full
-//      128-byte lines instead of 32 half-sectors of 32 different lines (L2 reduction throughput is per request);
-//      ws_tr = 0 keeps the row-major tile (row pitch BN floats).
-template <int BN, bool kExt, typename TmemDone>
-__device__ __forceinline__ void splitk_reduce_epilogue(const GemmParams& p, unsigned tile_id, uint32_t trow, int r,
+// ---- split-K hand-off (epilogue warpgroup, 128 threads): every CTA stores its fp32 partial tile into its own slice of
+//      the tile's workspace (slice = k-slice index); the last CTA to arrive (per-tile counter) adds the slices up in slice
+//      order -- the same order as the cluster exchange, so the result does not depend on which CTA finishes last --, runs
+//      the epilogue and re-zeroes the counter for the next launch.
+//      slice layout (p.ws_tr): float4 group g (= 4 columns) of row r lives at ((g * BM) + r) * 4 floats, so the 32 lanes of
+//      a warp (32 consecutive rows) touch 512 contiguous bytes per store / load -- four full 128-byte lines instead of 32
+//      half-sectors of 32 different lines; ws_tr = 0 keeps the row-major tile (row pitch BN floats).
+__device__ __forceinline__ void stage_ld32(const float* row, int c, uint32_t (&acc)[32]);
+template <int BN, bool kExt>
+__device__ __forceinline__ void splitk_reduce_epilogue(const GemmParams& p, unsigned tile_id, int sp, const float* trow, int r,
                                                        bool row_valid, long long grow, long long brow, int n0, int ncols_tile,
                                                        long long d_off, long long r_off, const float* sb, bool r_fast,
-                                                       long long r_row, TmemDone tmem_done) {
+                                                       long long r_row) {
     const int rs = p.ws_tr ? 4 : BN;             // floats between consecutive rows of one float4 group
     const int gs = p.ws_tr ? BM * 4 : 4;         // floats between consecutive float4 groups of one row
-    float* mine = p.ws + static_cast<size_t>(tile_id) * (BM * BN) + static_cast<size_t>(r) * rs;
-    ResidualChunk rc_cur;
+    float* slices = p.ws + static_cast<size_t>(tile_id) * p.splits * (BM * BN) + static_cast<size_t>(r) * rs;
+    float* mine = slices + static_cast<size_t>(sp) * (BM * BN);
 #pragma unroll 1
     for (int c = 0; c * 32 < ncols_tile; ++c) {
         uint32_t acc[32];
-        tmem_ld_32x32(trow + c * 32, acc);
-        tmem_ld_wait();
+        stage_ld32(trow, c, acc);
         if (row_valid) {
 #pragma unroll
             for (int j = 0; j < 32; j += 4)
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(mine + (c * 8 + (j >> 2)) * gs),
-                             "f"(__uint_as_float(acc[j])), "f"(__uint_as_float(acc[j + 1])),
-                             "f"(__uint_as_float(acc[j + 2])), "f"(__uint_as_float(acc[j + 3]))
-                             : "memory");
+                __stcg(reinterpret_cast<float4*>(mine + (c * 8 + (j >> 2)) * gs),
+                       make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]), __uint_as_float(acc[j + 2]),
+                                   __uint_as_float(acc[j + 3])));
         }
     }
-    tmem_done();
     __threadfence();
     asm volatile("bar.sync 1, 128;" ::: "memory");
     __shared__ unsigned s_last;
@@ -466,25 +461,26 @@ __device__ __forceinline__ void splitk_reduce_epilogue(const GemmParams& p, unsi
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
     const bool last = s_last != 0u;
-    asm volatile("bar.sync 1, 128;" ::: "memory");      // s_last is rewritten by the next tile of a persistent CTA
     if (!last) return;
     __threadfence();
     if (row_valid) {
-        // the sums of chunk c+1 are requested before chunk c is consumed: one L2 round trip for the whole tile instead of
-        // one per 32-column chunk (this CTA's tail is the critical path of the launch)
-        float4 v[8], vn[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = __ldcg(reinterpret_cast<const float4*>(mine + j * gs));
+        ResidualChunk rc_cur;
 #pragma unroll 1
         for (int c = 0; c * 32 < ncols_tile; ++c) {
-            if ((c + 1) * 32 < ncols_tile) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) vn[j] = __ldcg(reinterpret_cast<const float4*>(mine + ((c + 1) * 8 + j) * gs));
-            }
             const bool pre = r_fast && ncols_tile - c * 32 >= 32;
             if (pre) residual_prefetch(p, r_row + c * 32, rc_cur);
+            float4 v[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) __stcg(reinterpret_cast<float4*>(mine + (c * 8 + j) * gs), make_float4(0.f, 0.f, 0.f, 0.f));
+            for (int j = 0; j < 8; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+            for (int s2 = 0; s2 < p.splits; ++s2) {
+                const float* src = slices + static_cast<size_t>(s2) * (BM * BN);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float4 t = __ldcg(reinterpret_cast<const float4*>(src + (c * 8 + j) * gs));
+                    v[j].x += t.x; v[j].y += t.y; v[j].z += t.z; v[j].w += t.w;
+                }
+            }
             if (p.vec_ok && !p.d_transposed && ncols_tile - c * 32 >= 32) {
                 float f[32];
 #pragma unroll
@@ -505,31 +501,47 @@ __device__ __forceinline__ void splitk_reduce_epilogue(const GemmParams& p, unsi
                     }
                 }
             }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = vn[j];
         }
     }
     if (threadIdx.x == 64) p.counters[tile_id] = 0u;   // self-cleaning for the next launch
 }
 
-// kStages = 3: two CTAs per SM share the smem (large grids); kStages = 6: one CTA per SM with a deeper ring
-// (grids of <= one CTA per SM, where a single CTA must cover the whole TMA latency by itself).
+// Warp roles (384 threads, one CTA per SM):
+//   warpgroup 0 : thread 0 is the TMA producer; after the main loop all 128 threads run the epilogue, one output row each
+//   warpgroups 1, 2 : wgmma consumers, rows [0, 64) and [64, 128) of the tile, fp32 accumulators in registers
+// Once the last k-iteration has retired, the consumers park their accumulators in the (then idle) TMA ring as a row-major
+// fp32 tile of pitch BN + 4 floats (conflict-free 16-byte row reads), so the epilogue reads one row per thread.
+template <int BN>
+struct StageCfg {
+    static constexpr int kPitch = BN + 4;
+    static constexpr int kBytes = ((BM * kPitch * 4) + 1023) / 1024 * 1024;
+};
+
+// 32 consecutive accumulator columns of this thread's row from the staged tile
+__device__ __forceinline__ void stage_ld32(const float* row, int c, uint32_t (&acc)[32]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const float4 v = *reinterpret_cast<const float4*>(row + c * 32 + 4 * j);
+        acc[4 * j] = __float_as_uint(v.x); acc[4 * j + 1] = __float_as_uint(v.y);
+        acc[4 * j + 2] = __float_as_uint(v.z); acc[4 * j + 3] = __float_as_uint(v.w);
+    }
+}
+
 template <int BN, bool A_MN, bool B_MN, int kStages, bool kExt>
-__global__ void __launch_bounds__(kThreads, kStages <= 3 ? 2 : 1)
+__global__ void __launch_bounds__(kThreads, 1)
 cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ GemmParams p) {
     using Cfg = TileCfg<BN, kStages>;
+    using SCfg = StageCfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B needs 1 KiB alignment
+    float* stage = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)));
     const uint32_t bar_base = smem_base + kStages * Cfg::kStageBytes;
-    // barriers: full[kStages], empty[kStages], tmem_full; then the TMEM base address word
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-    const uint32_t tmem_full_bar = bar_base + 8u * (2 * kStages);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * kStages + 1);
 
     const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
     if (p.dbg_mode == 3) { pdl_sync(); return; }
     unsigned long long* dbg = p.dbg ? p.dbg + 8ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (dbg && threadIdx.x == 0) { dbg[0] = clock64(); dbg[7] = gtimer(); }
@@ -553,35 +565,26 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         m0 = m_tile * BM;
     }
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
+            mbar_init(empty_bar(s), 256);     // every consumer thread releases the stage
         }
-        mbar_init(tmem_full_bar, 1);
         mbar_fence_init();
         fence_proxy_async_smem();
     }
-    if (warp == 1) {
-        tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-    }
-    __syncwarp();   // warp 0 diverged on lane 0: reconverge before the aligned block barrier
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
     if (dbg && threadIdx.x == 0) dbg[1] = clock64();
-    pdl_sync();   // barrier init / TMEM allocation / descriptor prefetch above overlap the previous kernel's tail
+    pdl_sync();   // barrier init / descriptor prefetch above overlap the previous kernel's tail
 
     const int kiters_all = p.dbg_mode == 1 ? 0 : p.taps * p.kchunks;
     const int it0 = sp * p.kiters_per_split;
     const int it1 = min(kiters_all, it0 + p.kiters_per_split);
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             // ===================== TMA producer =====================
             for (int it = it0; it < it1; ++it) {
                 const int li = it - it0;
@@ -614,38 +617,54 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
             }
         }
-        if (p.cluster_sk) { __syncwarp(); cluster_sync_all(); cluster_sync_all(); }   // the two cluster barriers of the epilogue
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===================== MMA issuer =====================
-            for (int it = it0; it < it1; ++it) {
-                const int li = it - it0;
-                const int s = li % kStages;
-                const uint32_t ph = (li / kStages) & 1;
-                mbar_wait(full_bar(s), ph);
-                if (dbg && li == 0) dbg[2] = clock64();
-                tc_fence_after();
-                const uint32_t a_src = smem_base + s * Cfg::kStageBytes;
-                const uint32_t b_src = a_src + Cfg::kABytes;
-                const int kc = it % p.kchunks;
-                const int ksteps = (kc == p.kchunks - 1) ? p.ksteps_last : (BK / 16);
-                for (int k = 0; k < ksteps; ++k) {
-                    const uint64_t adesc = A_MN ? umma_smem_desc_sw128(a_src + k * 2048, 8192, 1024)
-                                                : umma_smem_desc_sw128(a_src + k * 32, 16, 1024);
-                    const uint64_t bdesc = B_MN ? umma_smem_desc_sw128(b_src + k * 2048, 8192, 1024)
-                                                : umma_smem_desc_sw128(b_src + k * 32, 16, 1024);
-                    umma_f16(tmem_base, adesc, bdesc, p.idesc, (li > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(empty_bar(s));  // frees this smem stage once the MMAs above retire
-            }
-            umma_commit(tmem_full_bar);
-            if (dbg) dbg[3] = clock64();
-        }
-        if (p.cluster_sk) { __syncwarp(); cluster_sync_all(); cluster_sync_all(); }
+        __syncwarp();
     } else {
-        // ===================== epilogue =====================
-        const int q = warp & 3;  // TMEM lane quarter this warp may read
-        const int r = q * 32 + lane;
+        // ===================== wgmma consumers =====================
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        const uint32_t a_half = static_cast<uint32_t>(wg - 1) * 8192u;     // this warpgroup's 64 rows of the A tile
+        for (int it = it0; it < it1; ++it) {
+            const int li = it - it0;
+            const int s = li % kStages;
+            mbar_wait(full_bar(s), (li / kStages) & 1);
+            if (dbg && li == 0 && threadIdx.x == 128) dbg[2] = clock64();
+            const uint32_t a_src = smem_base + s * Cfg::kStageBytes + a_half;
+            const uint32_t b_src = smem_base + s * Cfg::kStageBytes + Cfg::kABytes;
+            const int kc = it % p.kchunks;
+            const int ksteps = (kc == p.kchunks - 1) ? p.ksteps_last : (BK / 16);
+            wgmma_fence_regs(acc);
+            wgmma_fence();
+            for (int k = 0; k < ksteps; ++k) {
+                const uint64_t adesc = A_MN ? gmma_desc_sw128(a_src + k * 2048, 8192, 1024) : gmma_desc_sw128(a_src + k * 32, 16, 1024);
+                const uint64_t bdesc = B_MN ? gmma_desc_sw128(b_src + k * 2048, 8192, 1024) : gmma_desc_sw128(b_src + k * 32, 16, 1024);
+                wgmma_any<BN, A_MN, B_MN>(p.bf16 != 0, acc, adesc, bdesc, 1u);
+            }
+            wgmma_commit();
+            // keep one k-iteration of MMAs in flight: the previous stage is released once its group has retired
+            wgmma_wait<1>();
+            wgmma_fence_regs(acc);
+            if (li > 0) mbar_arrive(empty_bar((li - 1) % kStages));
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        if (it1 > it0) mbar_arrive(empty_bar((it1 - it0 - 1) % kStages));
+        if (dbg && threadIdx.x == 128) dbg[3] = clock64();
+        named_bar(4, 256);          // both warpgroups' MMAs have read the ring for the last time
+        const int l = threadIdx.x & 31, w = warp & 3;
+        float* srow = stage + ((wg - 1) * 64 + w * 16 + (l >> 2)) * SCfg::kPitch + 2 * (l & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            *reinterpret_cast<float2*>(srow + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(srow + 8 * SCfg::kPitch + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+    }
+    named_bar(2, kThreads);        // accumulator tile staged
+    if (p.cluster_sk && wg != 0) { cluster_sync_all(); cluster_sync_all(); }   // the two cluster barriers of the epilogue
+
+    if (wg == 0) {
+        // ===================== epilogue: one output row per thread =====================
+        const int r = threadIdx.x;
         bool row_valid;
         long long grow;
         if (p.conv) {
@@ -665,26 +684,24 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const long long d_off = (long long)zo * p.d_bs2 + (long long)zi * p.d_bs;
         const long long r_off = (long long)zo * p.r_bs2 + (long long)zi * p.r_bs;
         const int ncols_tile = min(BN, p.N - n0);
-        // bias row of this tile -> shared memory while the MMAs run (global bias loads in the store loop would each
-        // wait a full L2 round trip behind the previous chunk's stores)
+        // bias row of this tile -> shared memory (global bias loads in the store loop would each wait a full L2 round
+        // trip behind the previous chunk's stores)
         __shared__ __align__(16) float s_bias[BN + 8];
         const float* sb = nullptr;
         if (p.bias) {
             const long long tile_row0 = p.conv ? (((long long)img0 * p.out_h + oh0) * p.out_w + ow0) : (long long)m0;
             const long long brow0 = p.bias_row_div > 0 ? tile_row0 / p.bias_row_div : 0;
-            for (int i = threadIdx.x - 64; i < BN; i += 128) s_bias[i] = i < ncols_tile ? p.bias[brow0 * p.ldbias + n0 + i] : 0.f;
-            asm volatile("bar.sync 2, 128;" ::: "memory");
+            for (int i = threadIdx.x; i < BN; i += 128) s_bias[i] = i < ncols_tile ? p.bias[brow0 * p.ldbias + n0 + i] : 0.f;
+            named_bar(3, 128);
             if (brow == brow0) sb = s_bias;
         }
         // residual fast path: whole 32-column chunks, 16-byte aligned rows
         const bool r_fast = p.R && p.vec_ok && !p.d_transposed && row_valid;
         const long long r_row = r_off + grow * p.ldr + n0;
         ResidualChunk rc_cur, rc_next;
-        if (r_fast && p.splits == 1 && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);   // in flight during the MMAs
-        if (p.dbg_mode != 1) mbar_wait(tmem_full_bar, 0);
+        if (r_fast && p.splits == 1 && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);
         if (dbg && threadIdx.x == 64) dbg[4] = clock64();
-        tc_fence_after();
-        const uint32_t trow = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+        const float* trow = stage + r * SCfg::kPitch;
         if (p.dbg_mode == 1 || p.dbg_mode == 2) {
         } else if (p.splits == 1) {
 #pragma unroll 1
@@ -693,9 +710,8 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 if constexpr (kExt) {
                     if (p.glu) {
                         uint32_t acc2[32];
-                        tmem_ld_32x32(trow + c * 32, acc);
-                        tmem_ld_32x32(trow + c * 32 + 32, acc2);
-                        tmem_ld_wait();
+                        stage_ld32(trow, c, acc);
+                        stage_ld32(trow, c + 1, acc2);
                         if (row_valid) {
                             float fv[32], fg[32];
 #pragma unroll
@@ -706,10 +722,9 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         continue;
                     }
                 }
-                tmem_ld_32x32(trow + c * 32, acc);      // one TMEM round trip per 32 columns
+                stage_ld32(trow, c, acc);
                 const bool pre = r_fast && ncols_tile - c * 32 >= 32;
                 if (r_fast && ncols_tile - (c + 1) * 32 >= 32) residual_prefetch(p, r_row + (c + 1) * 32, rc_next);
-                tmem_ld_wait();
                 if (row_valid && p.vec_ok && !p.d_transposed && ncols_tile - c * 32 >= 32) {
                     float f[32];
 #pragma unroll
@@ -732,24 +747,24 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         } else if (p.cluster_sk) {
             // ---- split-K inside a thread-block cluster: the `splits` CTAs of this tile are the cluster (1,1,splits), rank =
             //      k-slice.  The 8-column groups of the tile are dealt round-robin to the CTAs (group g -> CTA g % S); every CTA
-            //      sends each group of its partial accumulator into the owner's shared memory (the TMA ring, idle once all
-            //      MMAs have retired), slot [sender][g / S][row] of 32 bytes, then sums its own groups over the S senders and
-            //      runs the epilogue for them.  Two cluster barriers (~0.2 us each) replace the L2 reductions, the
-            //      __threadfence, the arrival counter and the read-back of the global-workspace path (~4 us of round trips).
+            //      sends each group of its partial accumulator into the owner's exchange buffer (the part of the idle TMA ring
+            //      behind the staged tile), slot [sender][g / S][row] of 32 bytes, then sums its own groups over the S senders
+            //      and runs the epilogue for them.  Two cluster barriers replace the L2 reductions, the __threadfence, the
+            //      arrival counter and the read-back of the global-workspace path.
             const int S = p.splits;
             const int GI = (BN / 8 + S - 1) / S;                 // groups a CTA can own
+            const uint32_t xbuf = smem_base + SCfg::kBytes;
             fence_proxy_async_smem();                            // the ring was written / read through the async proxy
-            cluster_sync_all();                                  // #1: every CTA of the cluster has retired its MMAs
+            cluster_sync_all();                                  // #1: every CTA of the cluster has staged its accumulator
 #pragma unroll 1
             for (int c = 0; c * 32 < ncols_tile; ++c) {
                 uint32_t acc[32];
-                tmem_ld_32x32(trow + c * 32, acc);
-                tmem_ld_wait();
+                stage_ld32(trow, c, acc);
 #pragma unroll
                 for (int gq = 0; gq < 4; ++gq) {
                     const int g = c * 4 + gq;
                     if (g * 8 < ncols_tile)
-                        st_cluster_f32x8(smem_base + static_cast<uint32_t>(((sp * GI + g / S) * BM + r) * 32),
+                        st_cluster_f32x8(xbuf + static_cast<uint32_t>(((sp * GI + g / S) * BM + r) * 32),
                                          static_cast<uint32_t>(g % S), &acc[gq * 8]);
                 }
             }
@@ -760,7 +775,7 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll 4
                 for (int s2 = 0; s2 < S; ++s2) {
-                    const uint32_t a = smem_base + static_cast<uint32_t>(((s2 * GI + gi) * BM + r) * 32);
+                    const uint32_t a = xbuf + static_cast<uint32_t>(((s2 * GI + gi) * BM + r) * 32);
                     const float4 lo = ld_shared_f32x4(a), hi = ld_shared_f32x4(a + 16);
                     f[0] += lo.x; f[1] += lo.y; f[2] += lo.z; f[3] += lo.w;
                     f[4] += hi.x; f[5] += hi.y; f[6] += hi.z; f[7] += hi.w;
@@ -774,303 +789,12 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         } else {
             const unsigned tile_id = (static_cast<unsigned>(bz) * gridDim.y + m_tile) * gridDim.x + blockIdx.x;
-            splitk_reduce_epilogue<BN, kExt>(p, tile_id, trow, r, row_valid, grow, brow, n0, ncols_tile, d_off, r_off, sb,
-                                             r_fast, r_row, [] {});
+            splitk_reduce_epilogue<BN, kExt>(p, tile_id, sp, trow, r, row_valid, grow, brow, n0, ncols_tile, d_off, r_off, sb,
+                                             r_fast, r_row);
         }
+        if (dbg && threadIdx.x == 64) dbg[5] = clock64();
     }
-
-    if (dbg && threadIdx.x == 64) dbg[5] = clock64();
-    __syncwarp();   // warps 0/1 ran single-lane role loops: reconverge before the aligned block barrier
-    tc_fence_before();
-    __syncthreads();
     if (dbg && threadIdx.x == 0) dbg[6] = clock64();
-    if (warp == 1) {
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs on one TPC computes a 256 x BN tile with ONE
-// tcgen05.mma stream issued by the leader CTA.  Each CTA stages its own 128 rows of A and HALF of the B tile
-// (BN/2 columns); the MMA reads both halves, so per output element each SM pulls half as many B bytes out of
-// L2 as the single-CTA kernel -- the L2->SM ingest limit (~42 B/clk/SM) is what caps 128 x BN tiles at ~50 %
-// of the tensor peak on the large-M GEMMs (VAE 512^2/256^2 convolutions, CFG-batched inference).
-//   * TMA loads of both CTAs credit their bytes to the LEADER's full[] barrier (.cta_group::2, peer bit cleared);
-//   * tcgen05.commit.multicast frees the stage in both CTAs and publishes the accumulator to both epilogues;
-//   * each CTA's epilogue reads its own 128 TMEM lanes;
-//   * split-K (desc.splits > 1): the work items are (tile, k-slice) with the slice fastest, so the slices of one tile run
-//     on neighbouring clusters at the same time; each CTA of a pair reduces its 128 rows into its own workspace tile.
-// ---------------------------------------------------------------------------------------------
-template <int BN, int kStages>
-struct PairCfg {
-    static constexpr int kAccCols = BN <= 128 ? 128 : 256;      // TMEM columns of one accumulator
-    static constexpr int kTmemCols = 2 * kAccCols;              // two accumulators: epilogue(i) overlaps mainloop(i+1)
-    static constexpr int kABytes = BM * BK * 2;
-    static constexpr int kBBytes = (BN / 2) * BK * 2;          // this CTA's half of the B tile
-    static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-};
-
-// Persistent: gridDim.x = 2 * (number of clusters <= SMs / 2); cluster c works on tiles c, c + C, c + 2C, ... of the
-// (batch, m-pair, n-tile) space with n fastest (consecutive clusters share the same A rows in L2).  The shared-memory
-// ring and its phases run on across tiles; the accumulator alternates between two TMEM regions so the MMAs of tile i+1
-// start while the epilogue warps of both CTAs still drain tile i (tmem_full[acc] / tmem_empty[acc] barriers).
-template <int BN, bool B_MN, int kStages, bool kExt>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-cb_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ GemmParams p, int n_ntiles, int n_mpairs, int total_items) {
-    using Cfg = PairCfg<BN, kStages>;
-    constexpr int HN = BN / 2;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + kStages * Cfg::kStageBytes;
-    auto full_bar = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-    auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * kStages + a); };
-    auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * kStages + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * kStages + 4);
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int cid = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-        for (int s = 0; s < kStages; ++s) {
-            mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tfull_bar(a), 1);
-            mbar_init(tempty_bar(a), 2);        // one arrival per CTA of the pair (used on the leader only)
-        }
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    if (warp == 1) tmem_alloc_pair<Cfg::kTmemCols>(tmem_slot);
-    __syncwarp();
-    tc_fence_before();
-    cluster_sync_all();            // the peer's barriers exist before any remote arrive / complete_tx can reach them
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    pdl_sync();
-
-    const int kiters = p.taps * p.kchunks;
-    // tile t -> (batch z, m-pair, n-tile); this CTA's m tile = 2 * pair + rank
-    auto tile_coords = [&](int t, int& bz, int& m_tile, int& n0) {
-        const int nt = t % n_ntiles;
-        const int r = t / n_ntiles;
-        n0 = nt * BN;
-        m_tile = 2 * (r % n_mpairs) + (int)rank;
-        bz = r / n_mpairs;
-    };
-    auto tile_origin = [&](int m_tile, int& m0, int& ow0, int& oh0, int& img0) {
-        m0 = ow0 = oh0 = img0 = 0;
-        if (p.conv) {
-            const int tw = m_tile % p.tiles_w;
-            const int th = (m_tile / p.tiles_w) % p.tiles_h;
-            const int ti = m_tile / (p.tiles_w * p.tiles_h);
-            ow0 = tw * p.box_w;
-            oh0 = th * p.box_h;
-            img0 = ti * p.box_i;
-        } else {
-            m0 = m_tile * BM;
-        }
-    };
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ===================== TMA producer (both CTAs) =====================
-            int git = 0;
-            for (int w = cid; w < total_items; w += nclusters) {
-                const int t = w / p.splits, sp = w - t * p.splits;
-                const int it0 = sp * p.kiters_per_split, it1 = min(kiters, it0 + p.kiters_per_split);
-                int bz, m_tile, n0, m0, ow0, oh0, img0;
-                tile_coords(t, bz, m_tile, n0);
-                tile_origin(m_tile, m0, ow0, oh0, img0);
-                const int zi = bz % p.batch_inner, zo = bz / p.batch_inner;
-                const int nh = n0 + (int)rank * HN;          // this CTA's half of the B tile
-                for (int it = it0; it < it1; ++it, ++git) {
-                    const int s = git % kStages;
-                    const uint32_t ph = (git / kStages) & 1;
-                    mbar_wait(empty_bar(s), ph ^ 1u);
-                    if (leader) mbar_arrive_expect_tx(full_bar(s), 2u * (p.a_bytes + (unsigned)Cfg::kBBytes));
-                    const int tap = it / p.kchunks;
-                    const int kc = it - tap * p.kchunks;
-                    const uint32_t a_dst = smem_base + s * Cfg::kStageBytes;
-                    const uint32_t b_dst = a_dst + Cfg::kABytes;
-                    const int tap_b = p.flip_taps ? (p.taps - 1 - tap) : tap;
-                    if (p.conv) {
-                        const int r = tap / p.kw, sx = tap - r * p.kw;
-                        tma_load_4d_pair(a_dst, &tmA, full_bar(s), kc * BK, ow0 * p.stride + sx - p.pad_left,
-                                         oh0 * p.stride + r - p.pad_top, img0);
-                    } else {
-                        tma_load_4d_pair(a_dst, &tmA, full_bar(s), kc * BK, m0, zi, zo);
-                    }
-                    if (B_MN) {
-#pragma unroll
-                        for (int j = 0; j < HN / 64; ++j)
-                            tma_load_4d_pair(b_dst + j * 8192, &tmB, full_bar(s), nh + j * 64,
-                                             tap_b * p.b_tap_rows + kc * BK, zi, zo);
-                    } else {
-                        tma_load_4d_pair(b_dst, &tmB, full_bar(s), kc * BK, tap_b * p.b_tap_rows + nh, zi, zo);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && leader) {
-            // ===================== MMA issuer (leader CTA only) =====================
-            int git = 0, lt = 0;
-            for (int w = cid; w < total_items; w += nclusters, ++lt) {
-                const int sp = w % p.splits;
-                const int it0 = sp * p.kiters_per_split, it1 = min(kiters, it0 + p.kiters_per_split);
-                const int acc = lt & 1;
-                mbar_wait(tempty_bar(acc), (((unsigned)lt >> 1) & 1u) ^ 1u);      // both epilogues drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * Cfg::kAccCols);
-                for (int it = it0; it < it1; ++it, ++git) {
-                    const int s = git % kStages;
-                    const uint32_t ph = (git / kStages) & 1;
-                    mbar_wait(full_bar(s), ph);
-                    tc_fence_after();
-                    const uint32_t a_src = smem_base + s * Cfg::kStageBytes;
-                    const uint32_t b_src = a_src + Cfg::kABytes;
-                    const int kc = it % p.kchunks;
-                    const int ksteps = (kc == p.kchunks - 1) ? p.ksteps_last : (BK / 16);
-                    for (int k = 0; k < ksteps; ++k) {
-                        const uint64_t adesc = umma_smem_desc_sw128(a_src + k * 32, 16, 1024);
-                        const uint64_t bdesc = B_MN ? umma_smem_desc_sw128(b_src + k * 2048, 8192, 1024)
-                                                    : umma_smem_desc_sw128(b_src + k * 32, 16, 1024);
-                        umma_f16_pair(d_tmem, adesc, bdesc, p.idesc, (it > it0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit_pair(empty_bar(s));        // frees this stage in BOTH CTAs once the MMAs above retire
-                }
-                umma_commit_pair(tfull_bar(acc));
-            }
-        }
-    } else {
-        // ===================== epilogue (each CTA: its own 128 rows of every tile) =====================
-        const int q = warp & 3;
-        const int r = q * 32 + lane;
-        __shared__ __align__(16) float s_bias[BN + 8];
-        int lt = 0;
-        for (int w = cid; w < total_items; w += nclusters, ++lt) {
-            const int t = w / p.splits;
-            const int acc = lt & 1;
-            int bz, m_tile, n0, m0, ow0, oh0, img0;
-            tile_coords(t, bz, m_tile, n0);
-            tile_origin(m_tile, m0, ow0, oh0, img0);
-            const int zi = bz % p.batch_inner, zo = bz / p.batch_inner;
-            bool row_valid;
-            long long grow;
-            if (p.conv) {
-                const int per_img = p.box_h * p.box_w;
-                const int bi = r / per_img;
-                const int rem = r - bi * per_img;
-                const int bh = rem / p.box_w;
-                const int bw = rem - bh * p.box_w;
-                const int img = img0 + bi, oh = oh0 + bh, ow = ow0 + bw;
-                row_valid = (bi < p.box_i) && (img < p.img_n) && (oh < p.out_h) && (ow < p.out_w);
-                grow = ((long long)img * p.out_h + oh) * p.out_w + ow;
-            } else {
-                grow = m0 + r;
-                row_valid = grow < p.M;
-            }
-            const long long brow = p.bias_row_div > 0 ? grow / p.bias_row_div : 0;
-            const long long d_off = (long long)zo * p.d_bs2 + (long long)zi * p.d_bs;
-            const long long r_off = (long long)zo * p.r_bs2 + (long long)zi * p.r_bs;
-            const int ncols_tile = min(BN, p.N - n0);
-            const float* sb = nullptr;
-            if (p.bias) {
-                const long long tile_row0 = p.conv ? (((long long)img0 * p.out_h + oh0) * p.out_w + ow0) : (long long)m0;
-                const long long brow0 = p.bias_row_div > 0 ? tile_row0 / p.bias_row_div : 0;
-                for (int i = threadIdx.x - 64; i < BN; i += 128) s_bias[i] = i < ncols_tile ? p.bias[brow0 * p.ldbias + n0 + i] : 0.f;
-                asm volatile("bar.sync 2, 128;" ::: "memory");
-                if (brow == brow0) sb = s_bias;
-            }
-            const bool r_fast = p.R && p.vec_ok && !p.d_transposed && row_valid;
-            const long long r_row = r_off + grow * p.ldr + n0;
-            ResidualChunk rc_cur, rc_next;
-            if (r_fast && p.splits == 1 && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);
-            mbar_wait(tfull_bar(acc), ((unsigned)lt >> 1) & 1u);
-            tc_fence_after();
-            const uint32_t trow = tmem_base + (uint32_t)(acc * Cfg::kAccCols) + (static_cast<uint32_t>(q * 32) << 16);
-            if (p.splits > 1) {
-                // this CTA's 128 rows of the tile have their own workspace tile and arrival counter
-                splitk_reduce_epilogue<BN, kExt>(p, static_cast<unsigned>(t) * 2u + rank, trow, r, row_valid, grow, brow, n0,
-                                                 ncols_tile, d_off, r_off, sb, r_fast, r_row, [&] {
-                    tc_fence_before();                  // accumulator drained: hand it back before the L2 hand-off
-                    asm volatile("bar.sync 3, 128;" ::: "memory");
-                    if (threadIdx.x == 64) mbar_arrive_cluster(tempty_bar(acc), 0);
-                });
-                if (p.bias) asm volatile("bar.sync 2, 128;" ::: "memory");
-                continue;
-            }
-#pragma unroll 1
-            for (int c = 0; c * 32 < ncols_tile; ++c) {
-                uint32_t av[32];
-                if constexpr (kExt) {
-                    if (p.glu) {
-                        uint32_t av2[32];
-                        tmem_ld_32x32(trow + c * 32, av);
-                        tmem_ld_32x32(trow + c * 32 + 32, av2);
-                        tmem_ld_wait();
-                        if (c * 32 + 64 >= ncols_tile) {
-                            tc_fence_before();
-                            asm volatile("bar.sync 3, 128;" ::: "memory");
-                            if (threadIdx.x == 64) mbar_arrive_cluster(tempty_bar(acc), 0);
-                        }
-                        if (row_valid) {
-                            float fv[32], fg[32];
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) { fv[j] = __uint_as_float(av[j]) * p.alpha; fg[j] = __uint_as_float(av2[j]) * p.alpha; }
-                            epilogue_glu64(p, fv, fg, grow, n0 + c * 32, sb ? sb + c * 32 : nullptr);
-                        }
-                        ++c;
-                        continue;
-                    }
-                }
-                tmem_ld_32x32(trow + c * 32, av);
-                const bool pre = r_fast && ncols_tile - c * 32 >= 32;
-                if (r_fast && ncols_tile - (c + 1) * 32 >= 32) residual_prefetch(p, r_row + (c + 1) * 32, rc_next);
-                tmem_ld_wait();
-                if (c * 32 + 32 >= ncols_tile) {
-                    // last TMEM read of this accumulator: hand it back to the MMA issuer before the stores drain
-                    tc_fence_before();
-                    asm volatile("bar.sync 3, 128;" ::: "memory");
-                    if (threadIdx.x == 64) mbar_arrive_cluster(tempty_bar(acc), 0);
-                }
-                if (row_valid && p.vec_ok && !p.d_transposed && ncols_tile - c * 32 >= 32) {
-                    float f[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(av[j]) * p.alpha;
-                    epilogue_chunk32<kExt>(p, f, grow, brow, n0 + c * 32, d_off, r_off, pre ? &rc_cur : nullptr, sb ? sb + c * 32 : nullptr);
-                } else if (row_valid) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int nc = min(8, ncols_tile - c * 32 - g * 8);
-                        if (nc > 0) {
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(av[g * 8 + j]) * p.alpha;
-                            epilogue_group8<kExt>(p, f, grow, brow, n0 + c * 32 + g * 8, d_off, r_off, nc, nullptr, sb ? sb + c * 32 + g * 8 : nullptr);
-                        }
-                    }
-                }
-                rc_cur = rc_next;
-            }
-            if (p.bias) asm volatile("bar.sync 2, 128;" ::: "memory");      // s_bias is rewritten for the next tile
-        }
-    }
-    __syncwarp();
-    tc_fence_before();
-    cluster_sync_all();            // both CTAs are done with TMEM (and with each other's shared memory) before it is freed
-    if (warp == 1) tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1128,11 +852,10 @@ static int launch_se(const CUtensorMap& tA, const CUtensorMap& tB, const GemmPar
         attr_done = true;
     }
     if (p.cluster_sk) {
-        // the k-slices of a tile are one cluster (1,1,splits); the exchange buffer lives in the idle TMA ring
-        const int S = p.splits, GI = (BN / 8 + S - 1) / S;
+        // the k-slices of a tile are one cluster (1,1,splits); the exchange buffer lives in the idle TMA ring behind the
+        // staged accumulator tile (cluster_sk_fits)
+        const int S = p.splits;
         CB_REQUIRE(S >= 2 && S <= 16 && grid.z % S == 0, CB_ERR_ARG, "cb_gemm(cluster split-K): %d slices not in [2,16]", S);
-        CB_REQUIRE((long long)S * GI * BM * 32 <= (long long)kStages * Cfg::kStageBytes, CB_ERR_ARG,
-                   "cb_gemm(cluster split-K): exchange buffer (%d slices x %d groups) exceeds the %d-stage ring", S, GI, kStages);
         static bool np_done = false;
         if (S > 8 && !np_done) {
             CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
@@ -1155,62 +878,46 @@ static int launch_s(const CUtensorMap& tA, const CUtensorMap& tB, const GemmPara
                         : launch_se<BN, A_MN, B_MN, kStages, false>(tA, tB, p, grid, st);
 }
 
+// ring depth the launch below picks for this tile width / grid
+static int ring_stages(int bn, const GemmParams& p, long long ctas) {
+    if (bn == 256) return 4;
+    static const int env_force = getenv("CB_GEMM_STAGES") ? atoi(getenv("CB_GEMM_STAGES")) : 0;   // tuning aid
+    const int force = p.force_stages ? p.force_stages : env_force;
+    if (force == 3) return 3;
+    if (force == 6 || ctas <= device_sm_count()) return 6;
+    return 3;
+}
+// cluster split-K exchanges partial tiles through the part of the TMA ring behind the staged accumulator tile
+static bool cluster_sk_fits(int bn, int splits, int stages) {
+    const long long stage_bytes = ((long long)BM * (bn + 4) * 4 + 1023) / 1024 * 1024;
+    const long long ring = (long long)stages * (BM * BK * 2 + bn * BK * 2);
+    const long long gi = (bn / 8 + splits - 1) / splits;
+    return stage_bytes + (long long)splits * gi * BM * 32 <= ring;
+}
+
 template <int BN, bool A_MN, bool B_MN>
 static int launch(const CUtensorMap& tA, const CUtensorMap& tB, const GemmParams& p, dim3 grid, cudaStream_t st) {
     if constexpr (BN == 256) {
         return launch_s<BN, A_MN, B_MN, 4>(tA, tB, p, grid, st);   // 48 KiB stages: 4-deep ring, one CTA per SM
     } else {
         const long long ctas = (long long)grid.x * grid.y * grid.z;
-        static const int env_force = getenv("CB_GEMM_STAGES") ? atoi(getenv("CB_GEMM_STAGES")) : 0;   // tuning aid
-        const int force = p.force_stages ? p.force_stages : env_force;
-        if (force == 3) return launch_s<BN, A_MN, B_MN, 3>(tA, tB, p, grid, st);
-        if (force == 6 || ctas <= device_sm_count()) return launch_s<BN, A_MN, B_MN, 6>(tA, tB, p, grid, st);
+        if (ring_stages(BN, p, ctas) == 6) return launch_s<BN, A_MN, B_MN, 6>(tA, tB, p, grid, st);
         return launch_s<BN, A_MN, B_MN, 3>(tA, tB, p, grid, st);
     }
 }
 
-template <int BN, bool B_MN, bool kExt>
-static int launch_pair_e(const CUtensorMap& tA, const CUtensorMap& tB, const GemmParams& p, int n_mpairs, int n_ntiles,
-                         int batch, int max_ctas, cudaStream_t st) {
-    constexpr int kSt = 6;
-    using Cfg = PairCfg<BN, kSt>;
-    static bool attr_done = false;
-    auto kern = cb_gemm_pair_kernel<BN, B_MN, kSt, kExt>;
-    if (!attr_done) {
-        CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-        attr_done = true;
-    }
-    const long long total = (long long)n_mpairs * n_ntiles * batch * p.splits;       // work items: (tile, k-slice)
-    CB_REQUIRE(total < (1ll << 30), CB_ERR_ARG, "cb_gemm(pair): too many tiles");
-    // persistent grid: one cluster per SM pair, or fewer on request (desc.cta_pair = n >= 2: a throughput-bound producer
-    // that shares the device with a latency-bound chain leaves the other SMs to it)
-    const int cap = max_ctas >= 2 ? std::min(max_ctas, device_sm_count()) : device_sm_count();
-    const int clusters = (int)std::min<long long>(total, cap / 2);
-    dim3 grid((unsigned)(2 * clusters));
-    CB_LAUNCH((kern), grid, kThreads, Cfg::kSmemBytes, st, tA, tB, p, n_ntiles, n_mpairs, (int)total);
-    CB_CUDA(cudaGetLastError());
-    count_launches(1);
-    return 0;
-}
-
-template <int BN, bool B_MN>
-static int launch_pair(const CUtensorMap& tA, const CUtensorMap& tB, const GemmParams& p, int n_mpairs, int n_ntiles,
-                       int batch, int max_ctas, cudaStream_t st) {
-    return needs_ext(p) ? launch_pair_e<BN, B_MN, true>(tA, tB, p, n_mpairs, n_ntiles, batch, max_ctas, st)
-                        : launch_pair_e<BN, B_MN, false>(tA, tB, p, n_mpairs, n_ntiles, batch, max_ctas, st);
-}
-
-// Measured on B200 (tools/gemm_timeline.py): one SM pulls ~80 GB/s of operand tiles out of L2, i.e. a k-iteration of a
-// 128 x BN tile costs ~(128+BN)*128 B / 80 GB/s (0.45 us at BN=160) while its MMAs take 0.17 us; a split-K reduction
-// costs ~1 ns per 150 fp32 adds in L2 plus ~3 us of hand-off.  The tile width and the split are chosen to minimise
-// that estimate for the launch at hand.
+// Cost model of one launch: a k-iteration of a 128 x BN tile is taken to be bound by the operand bytes one SM pulls out
+// of L2 (~(128+BN)*128 B at ~80 GB/s per SM), a split-K reduction to cost ~1 ns per 150 fp32 adds in L2 plus ~3 us of
+// hand-off.  The constants are estimates, not measurements; the tile width and the split minimise the estimate for the
+// launch at hand, and the host autotuner (ops.py) times the real candidates.
 static double tile_time_us(int bn, long long tiles, int kiters, int sms) {
     const double t_iter = (128.0 + bn) * 128.0 / 80e3;          // us per k-iteration per CTA
     const long long waves = (tiles + sms - 1) / sms;
     return (double)waves * kiters * t_iter;
 }
 
-static int pick_bn(const cb_gemm_desc& d, int m_tiles, int kiters) {
+// requested = false: the library's own choice, ignoring desc.tile_n and CB_GEMM_BN
+static int pick_bn(const cb_gemm_desc& d, int m_tiles, int kiters, bool requested = true) {
     const int N = d.N;
     const int sms = device_sm_count();
     int cands[3];
@@ -1226,7 +933,7 @@ static int pick_bn(const cb_gemm_desc& d, int m_tiles, int kiters) {
         cands[nc++] = 64;
     }
     static const int env_bn = getenv("CB_GEMM_BN") ? atoi(getenv("CB_GEMM_BN")) : 0;   // tuning aid
-    const int force_bn = d.tile_n > 0 ? d.tile_n : env_bn;
+    const int force_bn = !requested ? 0 : (d.tile_n > 0 ? d.tile_n : env_bn);
     if (force_bn == 256 && N >= 256) return 256;    // 128x256 tile: only on request (per-shape autotuner / caller)
     for (int i = 0; i < nc; ++i)
         if (cands[i] == force_bn) return force_bn;
@@ -1342,11 +1049,10 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
         }
     }
 
-    // CTA-pair variant on request (desc.cta_pair = 1; the host autotuner decides): 256 x BN tiles, K-major A, no split-K
-    const bool pair = d.cta_pair >= 1 && !a_mn && m_tiles >= 2 && d.N >= 64;
-    int BN = pair ? ((d.tile_n == 128 || d.N <= 128) ? 128 : 256) : pick_bn(d, m_tiles, p.taps * p.kchunks);
+    // desc.cta_pair asks for large-M tiles of desc.tile_n; every tile is one CTA (sm_90 has no two-CTA MMA)
+    int BN = pick_bn(d, m_tiles, p.taps * p.kchunks);
     if (d.glu && BN % 64 != 0) BN = 128;        // (value, gate) column pairs live in 64-column groups
-    const int b_box_rows = pair ? BN / 2 : BN;
+    const int b_box_rows = BN;
     p.b_bytes = (unsigned)b_box_rows * BK * es;
     {
         const uint64_t brows_total = (uint64_t)(d.conv ? (int64_t)p.taps * d.b_tap_rows : (b_mn ? d.K : d.N));
@@ -1407,7 +1113,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
         static const int mode = getenv("CB_GEMM_DBG_MODE") ? atoi(getenv("CB_GEMM_DBG_MODE")) : 0;
         p.dbg_mode = mode;
     }
-    p.idesc = umma_idesc_f16(pair ? 2 * BM : BM, BN, d.ab_dtype == CB_BF16, a_mn, b_mn);
+    p.bf16 = d.ab_dtype == CB_BF16 ? 1 : 0;
     {
         const int des = d.d_dtype == CB_F32 ? 4 : 2;
         bool ok = ((reinterpret_cast<uintptr_t>(d.D) & 15u) == 0) && ((d.ldd * des) % 16 == 0) &&
@@ -1429,7 +1135,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
         p.vec32_ok = ok32 ? 1 : 0;
     }
 
-    // ---- split-K heuristic: fill the 148 SMs when the tile grid alone cannot (bs=1 low-resolution layers) ----
+    // ---- split-K heuristic: fill the SMs when the tile grid alone cannot (bs=1 low-resolution layers) ----
     p.force_stages = (d.stages == 3 || d.stages == 6) ? d.stages : 0;
     {
         static const int ws_tr = getenv("CB_GEMM_WS_TR") ? atoi(getenv("CB_GEMM_WS_TR")) : 1;   // A/B aid
@@ -1439,63 +1145,51 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
     p.kiters_per_split = p.taps * p.kchunks;
     {
         const int kiters = p.taps * p.kchunks;
-        const long long tiles = (long long)ceil_div(d.N, BN) * m_tiles * d.batch;
         const int sms = device_sm_count();
-        // (L2 reductions serialise per address, so split-K only pays when the output tile is small: <= 512 rows)
+        // The split is a function of the shape (or an explicit desc.splits) alone, never of the tile width a caller or the
+        // autotuner asks for: every configuration of a shape then adds its k-slices in the same order and the results are
+        // bit-identical whichever configuration wins the timing.
+        const int bn_s = pick_bn(d, m_tiles, kiters, false);
+        const long long tiles_s = (long long)ceil_div(d.N, bn_s) * m_tiles * d.batch;
         const long long counters_bytes = 65536;
         const long long avail = d.splitk_ws_bytes - counters_bytes;
-        const bool ws_ok = d.splitk_ws != nullptr && tiles <= counters_bytes / 4 && tiles * (long long)(BM * BN * 4) <= avail;
-        if (ws_ok && !d.glu && (d.splits > 0 || (tiles < sms && kiters >= 8))) {
+        // workspace bounds valid for every tile width: tiles <= ceil(N / 64) * ..., tiles * BN <= (N + 255) * ...
+        const long long tiles_max = (long long)ceil_div(d.N, 64) * m_tiles * d.batch;
+        const long long slice_bytes = (long long)(d.N + 255) * m_tiles * d.batch * BM * 4;
+        if (d.splitk_ws != nullptr && !d.glu && tiles_max <= counters_bytes / 4 &&
+            (d.splits > 0 || (tiles_s < sms && kiters >= 8))) {
             const double out_elems = (double)p.M * d.batch * d.N;
-            double best_t = tile_time_us(BN, tiles, kiters, sms);
+            double best_t = tile_time_us(bn_s, tiles_s, kiters, sms);
             int best_sp = 1;
             if (d.splits > 0) {
                 best_sp = d.splits < kiters ? d.splits : kiters;       // caller-tuned
             } else {
-                const int max_sp = (int)(sms / tiles) < 64 ? (int)(sms / tiles) : 64;
+                const int max_sp = (int)(sms / tiles_s) < 64 ? (int)(sms / tiles_s) : 64;
                 for (int sp = 2; sp <= max_sp; ++sp) {
                     const int per = ceil_div(kiters, sp);
                     if (per < 4) break;
-                    const double t = per * ((128.0 + BN) * 128.0 / 80e3) + out_elems * sp / 150e3 + 3.0;
+                    const double t = per * ((128.0 + bn_s) * 128.0 / 80e3) + out_elems * sp / 150e3 + 3.0;
                     if (t < best_t) { best_t = t; best_sp = sp; }
                 }
             }
             if (best_sp > 1) {
                 const int per = ceil_div(kiters, best_sp);
-                p.splits = ceil_div(kiters, per);
-                p.kiters_per_split = per;
-                p.counters = reinterpret_cast<unsigned*>(d.splitk_ws);
-                p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(d.splitk_ws) + counters_bytes);
+                const int splits = ceil_div(kiters, per);
+                if (slice_bytes * splits <= avail) {                       // one partial-tile slice per k-slice
+                    p.splits = splits;
+                    p.kiters_per_split = per;
+                    p.counters = reinterpret_cast<unsigned*>(d.splitk_ws);
+                    p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(d.splitk_ws) + counters_bytes);
+                }
             }
         }
     }
-    // split-K through distributed shared memory instead of the global workspace (desc.splitk_cluster, host autotuner)
-    p.cluster_sk = (d.splitk_cluster == 1 && !pair && p.splits >= 2 && p.splits <= 16 && p.dbg_mode == 0) ? 1 : 0;
+    // split-K through distributed shared memory instead of the global workspace (desc.splitk_cluster, host autotuner), where
+    // the exchange buffer fits the ring the launch runs with
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (pair) {
-        const int kiters = p.taps * p.kchunks;
-        const int mp = ceil_div(m_tiles, 2), nt = ceil_div(d.N, BN);
-        p.splits = 1;
-        p.kiters_per_split = kiters;
-        p.ws = nullptr;
-        p.counters = nullptr;
-        if (d.splits > 1 && !d.glu && d.splitk_ws != nullptr) {      // caller-tuned k-slices (the host autotuner)
-            const long long counters_bytes = 65536;
-            const long long cta_tiles = 2ll * mp * nt * d.batch;       // one workspace tile + counter per CTA of a pair
-            if (cta_tiles <= counters_bytes / 4 && cta_tiles * (long long)(BM * BN * 4) <= d.splitk_ws_bytes - counters_bytes) {
-                const int want = d.splits < kiters ? d.splits : kiters;
-                const int per = ceil_div(kiters, want);
-                p.splits = ceil_div(kiters, per);
-                p.kiters_per_split = per;
-                p.counters = reinterpret_cast<unsigned*>(d.splitk_ws);
-                p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(d.splitk_ws) + counters_bytes);
-            }
-        }
-        const int cap = d.cta_pair;      // 1 = whole device, n >= 2 = at most n CTAs
-        if (b_mn) return BN == 128 ? launch_pair<128, true>(tA, tB, p, mp, nt, d.batch, cap, st) : launch_pair<256, true>(tA, tB, p, mp, nt, d.batch, cap, st);
-        return BN == 128 ? launch_pair<128, false>(tA, tB, p, mp, nt, d.batch, cap, st) : launch_pair<256, false>(tA, tB, p, mp, nt, d.batch, cap, st);
-    }
     dim3 grid((unsigned)ceil_div(d.N, BN), (unsigned)m_tiles, (unsigned)(d.batch * p.splits));
+    p.cluster_sk = (d.splitk_cluster == 1 && p.splits >= 2 && p.splits <= 16 && p.dbg_mode == 0 &&
+                    cluster_sk_fits(BN, p.splits, ring_stages(BN, p, (long long)grid.x * grid.y * grid.z))) ? 1 : 0;
     if (!a_mn && !b_mn) {
         if (BN == 64) return launch<64, false, false>(tA, tB, p, grid, st);
         if (BN == 128) return launch<128, false, false>(tA, tB, p, grid, st);

@@ -38,11 +38,24 @@ __device__ __forceinline__ float silu_grad(float z) {
     return s * (1.0f + z * (1.0f - s));
 }
 
-// Per-group accumulation into shared memory.  Float atomics on shared memory are compare-and-swap loops, so letting
-// every lane hit the (few) group addresses serialises the whole CTA: lanes of a warp that hold the same group (a
-// contiguous run, since channel pairs are lane-consecutive) first add up with shuffles and only the run's first lane
-// issues the atomic.  Must be called by all live lanes of the warp (uniform control flow).
+// Per-group accumulation into shared memory in a fixed order, so that the statistics are bit-identical from run to run:
+// lanes of a warp that hold the same group add up with shuffles (a tree over a contiguous run, else in lane order), the
+// run's first lane adds the result into its warp's slot, and group_acc_flush() adds the slots into s_a / s_b in warp
+// order.  group_accumulate must be called by all live lanes of the warp (uniform control flow); group_acc_begin() and
+// group_acc_flush() by every thread of the block.
+constexpr int kGnSlotWarps = 32;          // up to 1024 threads
+struct GnSlots { float2 v[kGnSlotWarps][64]; };
+__device__ __forceinline__ GnSlots& gn_slots() {
+    __shared__ GnSlots s;
+    return s;
+}
+__device__ __forceinline__ void group_acc_begin() {
+    float2* v = &gn_slots().v[0][0];
+    for (int i = threadIdx.x; i < kGnSlotWarps * 64; i += blockDim.x) v[i] = make_float2(0.f, 0.f);
+    __syncthreads();
+}
 __device__ __forceinline__ void group_accumulate(float* s_a, float* s_b, int g, float v1, float v2) {
+    (void)s_a; (void)s_b;
     const unsigned act = __activemask();
     const unsigned peers = __match_any_sync(act, g);
     const int lane = threadIdx.x & 31;
@@ -56,13 +69,51 @@ __device__ __forceinline__ void group_accumulate(float* s_a, float* s_b, int g, 
             const float t2 = __shfl_down_sync(act, v2, off);
             if (lane + off <= last) { v1 += t1; v2 += t2; }
         }
-        if (lane == first) { atomicAdd(&s_a[g], v1); atomicAdd(&s_b[g], v2); }
     } else {
-        atomicAdd(&s_a[g], v1);
-        atomicAdd(&s_b[g], v2);
+        float t1 = 0.f, t2 = 0.f;
+        for (int l = 0; l < 32; ++l) {
+            if (!((act >> l) & 1u)) continue;
+            const float u1 = __shfl_sync(act, v1, l), u2 = __shfl_sync(act, v2, l);
+            if ((peers >> l) & 1u) { t1 += u1; t2 += u2; }
+        }
+        v1 = t1; v2 = t2;
     }
+    if (lane == first) {
+        float2& sl = gn_slots().v[threadIdx.x >> 5][g];
+        sl = make_float2(sl.x + v1, sl.y + v2);
+    }
+    __syncwarp(act);
+}
+// after a __syncthreads(): s_a[g] += sum over warps (in warp order) of the slots, for g < n
+__device__ __forceinline__ void group_acc_flush(float* s_a, float* s_b, int n) {
+    if ((int)threadIdx.x < n) {
+        float a = 0.f, b = 0.f;
+        const int nw = (blockDim.x + 31) >> 5;
+        for (int w = 0; w < nw; ++w) { const float2 v = gn_slots().v[w][threadIdx.x]; a += v.x; b += v.y; }
+        s_a[threadIdx.x] += a;
+        s_b[threadIdx.x] += b;
+    }
+    __syncthreads();
+}
+// streaming two-kernel path: the statistics kernel publishes one (sum, sum2) partial per CTA and group, the apply kernel
+// (same grid) adds them up in CTA order
+__device__ __forceinline__ void publish_block_partials(double* ws, const float* s_a, const float* s_b, int G) {
+    if ((int)threadIdx.x < G)
+        reinterpret_cast<float2*>(ws)[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * G + threadIdx.x] =
+            make_float2(s_a[threadIdx.x], s_b[threadIdx.x]);
+}
+__device__ __forceinline__ double2 sum_block_partials(const double* ws, int G, int g) {
+    const float2* part = reinterpret_cast<const float2*>(ws);
+    double a = 0.0, b = 0.0;
+    for (int k = 0; k < (int)gridDim.x; ++k) {
+        const float2 v = part[((size_t)blockIdx.y * gridDim.x + k) * G + g];
+        a += v.x;
+        b += v.y;
+    }
+    return make_double2(a, b);
 }
 
+constexpr int kGnMaxDynSmem = 184 * 1024;  // dynamic shared memory of the staged variants (+ GnSlots + statics <= 227 KiB)
 constexpr int kGnThreads = 256;           // upper bound; the launch uses PW*RY threads (see gn_shape)
 constexpr int kGnFusedThreads = 1024;     // fused kernels: one CTA per SM, so fill it (PW x up-to-1024/PW row lanes)
 constexpr int kGnMaxChunks = 8;           // channel-pair chunks per thread: C <= 2*PW*8
@@ -82,7 +133,7 @@ static inline GnShape gn_shape(int C) {
     return s;
 }
 
-// ---- GroupNorm statistics: ws[(n*G+g)*2 + {0,1}] += {sum, sumsq} (fp64) ---------------------------
+// ---- GroupNorm statistics: one (sum, sumsq) partial per CTA and group into ws (publish_block_partials) ----------
 template <typename TX>
 __global__ void __launch_bounds__(kGnThreads)
 gn_stats_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, int C, int G, int rows_per_block, int PW,
@@ -95,6 +146,7 @@ gn_stats_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, int C
     const int r1 = min(HW, r0 + rows_per_block);
     const int cpg = C / G;
     if (threadIdx.x < 64) { s_sum[threadIdx.x] = 0.f; s_sq[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     float a1[kGnMaxChunks], a2[kGnMaxChunks];
 #pragma unroll
@@ -120,10 +172,8 @@ gn_stats_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, int C
         }
     }
     __syncthreads();
-    if (threadIdx.x < G) {
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 0], (double)s_sum[threadIdx.x]);
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 1], (double)s_sq[threadIdx.x]);
-    }
+    group_acc_flush(s_sum, s_sq, 64);
+    publish_block_partials(ws, s_sum, s_sq, G);
 }
 
 // ---- GroupNorm apply: y = act((x-mean)*rstd*gamma+beta) ---------------------------------------------
@@ -140,8 +190,9 @@ gn_apply_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* __res
     const int cpg = C / G;
     if (threadIdx.x < G) {
         const double cnt = (double)HW * cpg;
-        const double m = ws[((size_t)n * G + threadIdx.x) * 2] / cnt;
-        double var = ws[((size_t)n * G + threadIdx.x) * 2 + 1] / cnt - m * m;
+        const double2 sums = sum_block_partials(ws, G, threadIdx.x);
+        const double m = sums.x / cnt;
+        double var = sums.y / cnt - m * m;
         if (var < 0) var = 0;
         const float rs = (float)(1.0 / sqrt(var + (double)eps));
         s_mean[threadIdx.x] = (float)m;
@@ -221,6 +272,7 @@ gn_stats_tma_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, i
         fence_proxy_async_smem();
     }
     if (threadIdx.x < 64) { s_sum[threadIdx.x] = 0.f; s_sq[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     pdl_sync();
     float a1[kGnMaxChunks], a2[kGnMaxChunks];
@@ -251,10 +303,8 @@ gn_stats_tma_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, i
         }
     }
     __syncthreads();
-    if (threadIdx.x < G) {
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 0], (double)s_sum[threadIdx.x]);
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 1], (double)s_sq[threadIdx.x]);
-    }
+    group_acc_flush(s_sum, s_sq, 64);
+    publish_block_partials(ws, s_sum, s_sq, G);
 }
 
 template <typename TX, typename TY>
@@ -278,8 +328,9 @@ gn_apply_tma_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* _
     pdl_sync();
     if (threadIdx.x < G) {
         const double cnt = (double)HW * cpg;
-        const double m = ws[((size_t)n * G + threadIdx.x) * 2] / cnt;
-        double var = ws[((size_t)n * G + threadIdx.x) * 2 + 1] / cnt - m * m;
+        const double2 sums = sum_block_partials(ws, G, threadIdx.x);
+        const double m = sums.x / cnt;
+        double var = sums.y / cnt - m * m;
         if (var < 0) var = 0;
         const float rs = (float)(1.0 / sqrt(var + (double)eps));
         s_mean[threadIdx.x] = (float)m;
@@ -339,6 +390,7 @@ gn_bwd_stats_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
     const int tx = threadIdx.x % PW, ty = threadIdx.x / PW;
     const int cpg = C / G;
     if (threadIdx.x < 64) { s_1[threadIdx.x] = 0.f; s_2[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     const int r0 = blockIdx.x * rows_per_block;
     const int r1 = min(HW, r0 + rows_per_block);
@@ -366,10 +418,8 @@ gn_bwd_stats_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
         group_accumulate(s_1, s_2, g, a1, a2);
     }
     __syncthreads();
-    if (threadIdx.x < G) {
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 0], (double)s_1[threadIdx.x]);
-        atomicAdd(&ws[((size_t)n * G + threadIdx.x) * 2 + 1], (double)s_2[threadIdx.x]);
-    }
+    group_acc_flush(s_1, s_2, 64);
+    publish_block_partials(ws, s_1, s_2, G);
 }
 
 // ---- GroupNorm backward apply: dx (+)= rstd*(dz*gamma - s1/cnt - xhat*s2/cnt) ----------------------------
@@ -386,8 +436,9 @@ gn_bwd_apply_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
     const int cpg = C / G;
     if (threadIdx.x < G) {
         const double cnt = (double)HW * cpg;
-        s_1[threadIdx.x] = (float)(ws[((size_t)n * G + threadIdx.x) * 2] / cnt);
-        s_2[threadIdx.x] = (float)(ws[((size_t)n * G + threadIdx.x) * 2 + 1] / cnt);
+        const double2 sums = sum_block_partials(ws, G, threadIdx.x);
+        s_1[threadIdx.x] = (float)(sums.x / cnt);
+        s_2[threadIdx.x] = (float)(sums.y / cnt);
     }
     __syncthreads();
     const int r0 = blockIdx.x * rows_per_block;
@@ -517,6 +568,7 @@ gn_fused_fwd_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* _
         fence_proxy_async_smem();
     }
     if (threadIdx.x < 64) { s_a[threadIdx.x] = 0.f; s_b[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     pdl_sync();
     if (threadIdx.x == 0 && r1 > r0) {
@@ -548,6 +600,7 @@ gn_fused_fwd_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* _
         }
     }
     __syncthreads();
+    group_acc_flush(s_a, s_b, 64);
     float2* part = reinterpret_cast<float2*>(ws);
     publish_partials(part, s_a, s_b, G);
     grid_arrive_and_wait(counter, gridDim.x * gridDim.y);
@@ -611,6 +664,7 @@ gn_fused_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
         fence_proxy_async_smem();
     }
     if (threadIdx.x < 64) { s_1[threadIdx.x] = 0.f; s_2[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     pdl_sync();
     const size_t base = ((size_t)n * HW) * C;
@@ -644,6 +698,7 @@ gn_fused_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
         group_accumulate(s_1, s_2, g, a1, a2);
     }
     __syncthreads();
+    group_acc_flush(s_1, s_2, 64);
     float2* part = reinterpret_cast<float2*>(ws);
     publish_partials(part, s_1, s_2, G);
     grid_arrive_and_wait(counter, gridDim.x * gridDim.y);
@@ -779,6 +834,7 @@ gn_cluster_fwd_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float*
     const int cpg = C / G, cw = gpc * cpg, nq = cw >> 2, c0 = slab * cw;
     const int r0 = rank * rows_per_cta, r1 = min(HW, r0 + rows_per_cta);
     if (threadIdx.x < 32) { s_a[threadIdx.x] = 0.f; s_b[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     pdl_sync();
     const GnClMap m = gn_cl_map(nq, cpg);
@@ -798,6 +854,8 @@ gn_cluster_fwd_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float*
         group_accumulate(s_a, s_b, m.gA, a1, a2);
         group_accumulate(s_a, s_b, m.gB, b1, b2);
     }
+    __syncthreads();
+    group_acc_flush(s_a, s_b, 32);
     gn_cl_allreduce(s_a, s_b, s_recv, s_t1, s_t2, gpc, S, rank);
     if (threadIdx.x < gpc) {
         const double cnt = (double)HW * cpg;
@@ -850,6 +908,7 @@ gn_cluster_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const
     const int c0 = slab * cw;
     const int r0 = rank * rows_per_cta, r1 = min(HW, r0 + rows_per_cta);
     if (threadIdx.x < 32) { s_a[threadIdx.x] = 0.f; s_b[threadIdx.x] = 0.f; }
+    group_acc_begin();
     __syncthreads();
     pdl_sync();
     const GnClMap m = gn_cl_map(nq, cpg);
@@ -891,6 +950,8 @@ gn_cluster_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const
         group_accumulate(s_a, s_b, m.gA, a1, a2);
         group_accumulate(s_a, s_b, m.gB, b1, b2);
     }
+    __syncthreads();
+    group_acc_flush(s_a, s_b, 32);
     gn_cl_allreduce(s_a, s_b, s_recv, s_t1, s_t2, gpc, S, rank);
     if (threadIdx.x < gpc) {
         const double cnt = (double)HW * cpg;
@@ -942,7 +1003,7 @@ static inline bool gn_cluster_plan(int N, int HW, int C, int G, size_t bytes_per
         if (S > HW) S = 1;
         const int rows = ceil_div(HW, S);
         const size_t smem = (((size_t)rows * cw * bytes_per_elem) + 255) & ~(size_t)127;
-        if (smem > 200 * 1024) continue;
+        if (smem > kGnMaxDynSmem) continue;
         out->S = S; out->gpc = gpc; out->rows_per_cta = rows; out->smem = smem;
         return true;
     }
@@ -1054,9 +1115,11 @@ ln_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const float* 
     }
 }
 
-static inline int gn_rows_per_block(int HW, int N) {
+// CTAs per image whose (sum, sumsq) partials (float2 per group) fit the caller's workspace
+static inline int gn_max_blocks(int N, int G) { return std::max(1, (int)((CB_GN_WS_BYTES - 8) / (8 * (size_t)G * N))); }
+static inline int gn_rows_per_block(int HW, int N, int G) {
     const int target_blocks = 8 * device_sm_count();     // 256-thread blocks: 8 per SM keep 2048 threads x 8 loads in flight
-    int per_img = ceil_div(target_blocks, N);
+    int per_img = std::min(ceil_div(target_blocks, N), gn_max_blocks(N, G));
     if (per_img < 1) per_img = 1;
     int rpb = ceil_div(HW, per_img);
     if (rpb < 1) rpb = 1;
@@ -1118,7 +1181,7 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
                 auto kern = gn_cluster_fwd_kernel<TX, TY>;
                 static bool set = false;
                 if (!set) {
-                    le = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+                    le = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem);
                     if (le == cudaSuccess) le = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
                     set = le == cudaSuccess;
                 }
@@ -1146,14 +1209,14 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
         if (nb >= 1 && allow_fused) {
             const int rpbf = ceil_div(HW, nb);
             const size_t smem = (size_t)rpbf * C * xes;
-            if (smem <= 200 * 1024 && ((size_t)C * xes) % 16 == 0) {
+            if (smem <= kGnMaxDynSmem && ((size_t)C * xes) % 16 == 0) {
                 dim3 gridf(ceil_div(HW, rpbf), N);
                 CB_REQUIRE((size_t)gridf.x * N * G * 8 <= CB_GN_WS_BYTES - 8, CB_ERR_ARG, "groupnorm: workspace too small");
                 const int ryf = std::max(1, std::min(rpbf, kGnFusedThreads / gs.pw));
                 CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY, {
                     auto kern = gn_fused_fwd_kernel<TX, TY>;
                     static size_t max_set = 0;
-                    if (smem > max_set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); max_set = 200 * 1024; }
+                    if (smem > max_set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem)); max_set = kGnMaxDynSmem; }
                     CB_LAUNCH((kern), gridf, gs.pw * ryf, smem, st, (const TX*)x, (TY*)y, gamma, beta, ws, counter, mean_out, rstd_out, HW, C, G, eps, act_silu, rpbf, gs.pw, ryf, gs.chunks);
                 }));
                 CB_CUDA(cudaGetLastError());
@@ -1162,7 +1225,6 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
             }
         }
     }
-    CB_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * N * G, st));
     {
         // streaming (TMA-staged) variant: rows are 16-byte multiples and a chunk of them fits one 32 KiB stage
         const int xes = x_dtype == CB_F32 ? 4 : 2;
@@ -1170,7 +1232,7 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
         const int rpc = (int)(kGnTmaChunkBytes / row_bytes);
         if (row_bytes % 16 == 0 && rpc >= 1) {
             const int ctas = cta_cap > 0 ? std::min(cta_cap, 2 * device_sm_count()) : 2 * device_sm_count();
-            const int nb = std::max(1, ctas / N);
+            const int nb = std::max(1, std::min(ctas / N, gn_max_blocks(N, G)));
             const int rpbt = ceil_div(HW, nb);
             dim3 gridt(ceil_div(HW, rpbt), N);
             const size_t smem = (size_t)kGnTmaStages * kGnTmaChunkBytes;
@@ -1191,7 +1253,7 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
             return 0;
         }
     }
-    const int rpb = gn_rows_per_block(HW, N);
+    const int rpb = gn_rows_per_block(HW, N, G);
     dim3 grid(ceil_div(HW, rpb), N);
     CB_DISPATCH_2(x_dtype, TX,CB_LAUNCH((gn_stats_kernel<TX>), grid, nthr, 0, st, (const TX*)x, ws, HW, C, G, rpb, gs.pw, gs.ry, gs.chunks));
     CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY,
@@ -1224,7 +1286,7 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
                 auto kern = gn_cluster_bwd_kernel<TX, TG, TDX>;                                                                   \
                 static bool set = false;                                                                                          \
                 if (!set) {                                                                                                       \
-                    le = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);                     \
+                    le = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem);                     \
                     if (le == cudaSuccess) le = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);    \
                     set = le == cudaSuccess;                                                                                      \
                 }                                                                                                                 \
@@ -1252,7 +1314,7 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
             const int rpbf = ceil_div(HW, nb);
             const int xes = x_dtype == CB_F32 ? 4 : 2, ges = dy_dtype == CB_F32 ? 4 : 2;
             const size_t smem = (((size_t)rpbf * C * xes + 127) & ~(size_t)127) + (size_t)rpbf * C * ges;   // staged x + dy
-            if (smem <= 200 * 1024 && ((size_t)C * xes) % 16 == 0 && ((size_t)C * ges) % 16 == 0) {
+            if (smem <= kGnMaxDynSmem && ((size_t)C * xes) % 16 == 0 && ((size_t)C * ges) % 16 == 0) {
                 dim3 gridf(ceil_div(HW, rpbf), N);
                 CB_REQUIRE((size_t)gridf.x * N * G * 8 <= CB_GN_WS_BYTES - 8, CB_ERR_ARG, "groupnorm: workspace too small");
                 const int ryf = std::max(1, std::min(rpbf, kGnFusedThreads / gs.pw));
@@ -1260,7 +1322,7 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
                 CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(dy_dtype, TG, {                                                              \
                     auto kern = gn_fused_bwd_kernel<TX, TG, TDX>;                                                                     \
                     static bool set = false;                                                                                         \
-                    if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); set = true; } \
+                    if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem)); set = true; } \
                     CB_LAUNCH((kern), gridf, gs.pw * ryf, smem, st, (const TG*)dy, (const TX*)x, gamma, beta, mean, rstd, ws, counter, (TDX*)dx, (TG*)dx_lp, HW, C, G, act_silu, accumulate, rpbf, gs.pw, ryf, gs.chunks); \
                 }))
                 if (dx_dtype == CB_F32) { CB_GN_BWD_FUSED(float); } else { CB_GN_BWD_FUSED(TG); }
@@ -1271,8 +1333,7 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
             }
         }
     }
-    CB_CUDA(cudaMemsetAsync(ws, 0, sizeof(double) * 2 * N * G, st));
-    const int rpb = gn_rows_per_block(HW, N);
+    const int rpb = gn_rows_per_block(HW, N, G);
     dim3 grid(ceil_div(HW, rpb), N);
     CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(dy_dtype, TG,
 CB_LAUNCH((gn_bwd_stats_kernel<TX, TG>), grid, nthr, 0, st, (const TG*)dy, (const TX*)x, gamma, beta, mean, rstd, ws, HW, C, G, act_silu, rpb, gs.pw, gs.ry, gs.chunks)));

@@ -1,4 +1,4 @@
-"""CosFace iresnet100 forward (eval, no grad) on the sm_100a kernels.
+"""CosFace iresnet100 forward (eval, no grad) on the sm_90a kernels.
 
 Mirrors ldm/modules/id_embedding/iresnet.py:166-181 (IResNet.forward) and :26-64 (IBasicBlock):
     bn1 -> conv3x3 -> bn2 -> PReLU -> conv3x3(stride) -> bn3  (+ identity | conv1x1(stride)+bn)

@@ -45,7 +45,7 @@ class AutoencoderKL(nn.Module):
     def _dev(self):
         dev = self.quant_conv.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("celebbasis_b200 AutoencoderKL runs on sm_100a only (no CPU fallback)")
+            raise RuntimeError("celebbasis_b200 AutoencoderKL runs on sm_90a only (no CPU fallback)")
         return dev
 
     def encode(self, x):

@@ -5,4 +5,4 @@ The PLMS sampler is not on the CelebBasis hot path (SURVEY.md section 2: the ref
 
 class PLMSSampler:
     def __init__(self, model, schedule="linear", **kwargs):
-        raise NotImplementedError("PLMSSampler is out of scope for the B200 path: use DDIMSampler (--plms off)")
+        raise NotImplementedError("PLMSSampler is out of scope for the H100 path: use DDIMSampler (--plms off)")

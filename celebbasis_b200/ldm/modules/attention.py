@@ -4,7 +4,7 @@
 The classes keep the reference's constructor arguments and parameter names (so SD-v1 checkpoints load by key).
 Inside a UNetModel they are parameter containers: the UNet engine (celebbasis_b200/unet_engine.py) reads their
 weights and runs the fused kernels.  CrossAttention.forward is also usable stand-alone (inference, no grad): it
-runs q/k/v projection, scaled-dot-product softmax and out-projection on the tcgen05 GEMM + softmax kernels.
+runs q/k/v projection, scaled-dot-product softmax and out-projection on the wgmma GEMM + softmax kernels.
 """
 import torch
 from torch import nn
@@ -73,7 +73,7 @@ class CrossAttention(nn.Module):
         """x: (B, N, query_dim); context: (B, M, context_dim) or None (self-attention).  Returns (B, N, query_dim)."""
         assert mask is None, "the mask path of attention.py:182-186 is unused by CelebBasis"
         if not x.is_cuda:
-            raise RuntimeError("celebbasis_b200 CrossAttention runs on sm_100a only (no CPU fallback)")
+            raise RuntimeError("celebbasis_b200 CrossAttention runs on sm_90a only (no CPU fallback)")
         dt = torch.float16
         wq, wk, wv, wo, bo = self._pack(dt)
         B, N, _ = x.shape

@@ -141,7 +141,7 @@ class UNetModel(nn.Module):
     def engine(self, dtype=torch.float16):
         dev = self.time_embed[0].weight.device
         if dev.type != "cuda":
-            raise RuntimeError("celebbasis_b200 UNetModel runs on sm_100a only (no CPU fallback): move it to cuda")
+            raise RuntimeError("celebbasis_b200 UNetModel runs on sm_90a only (no CPU fallback): move it to cuda")
         if self._engine is None or self._engine.dev != dev or self._engine.dt != dtype:
             self._engine = UNetEngine(self.engine_config(), self.state_dict(), dev, dtype=dtype)
             self.__dict__.pop("_graphs", None)

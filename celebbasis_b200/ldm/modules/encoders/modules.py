@@ -121,7 +121,7 @@ class _AddPosFn(torch.autograd.Function):
 
 
 class FrozenCLIPEmbedder(AbstractEncoder):
-    """Uses the CLIP transformer encoder for text (Hugging Face layout), B200-native arithmetic."""
+    """Uses the CLIP transformer encoder for text (Hugging Face layout), H100-native arithmetic."""
 
     def __init__(self, version="openai/clip-vit-large-patch14", device="cuda", max_length=77,
                  celeb_txt="./infer_images/wiki_names_v2.txt", use_celeb=False, use_svd=False, n_components: int = 512,
@@ -172,7 +172,7 @@ class FrozenCLIPEmbedder(AbstractEncoder):
         tm = self.transformer.text_model
         dev = tm.final_layer_norm.weight.device
         if dev.type != "cuda":
-            raise RuntimeError("celebbasis_b200 FrozenCLIPEmbedder runs on sm_100a only (no CPU fallback)")
+            raise RuntimeError("celebbasis_b200 FrozenCLIPEmbedder runs on sm_90a only (no CPU fallback)")
         if self._engine is None or self._engine.dev != dev or self._engine.dt != dtype:
             self._engine = CLIPTextEngine(self.transformer.state_dict(), dev, dtype=dtype, heads=tm.heads, eps=tm.eps)
         return self._engine

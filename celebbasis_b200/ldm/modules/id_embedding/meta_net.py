@@ -87,7 +87,7 @@ class MetaIdNet(nn.Module):
     def face_engine(self):
         dev = self.stylegan_mlp.net[0].weight.device
         if dev.type != "cuda":
-            raise RuntimeError("celebbasis_b200 MetaIdNet runs on sm_100a only (no CPU fallback)")
+            raise RuntimeError("celebbasis_b200 MetaIdNet runs on sm_90a only (no CPU fallback)")
         if self._face_engine is None or self._face_engine.dev != dev:
             self._face_engine = IResNetEngine(self.id_model.state_dict(), dev)
         return self._face_engine

@@ -1,6 +1,6 @@
 """ctypes binding of libcelebbasis_b200.so (the C-ABI in include/celebbasis_b200.h).
 
-There is deliberately NO fallback: if the shared object is missing or the device is not sm_100
+There is deliberately NO fallback: if the shared object is missing or the device is not sm_90
 the product path raises.  (tests/ and bench.py's cpu_baseline are the only users of oracle/.)
 """
 import ctypes

@@ -71,19 +71,16 @@ def _splitk_workspace(device):
 # shape times the candidates on the device (CUDA-graph replay of 8 launches each, output redirected to scratch) and
 # later launches -- including the ones captured into the step graph -- pass the winner in desc.tile_n / desc.splits.
 AUTOTUNE = os.environ.get("CB_GEMM_AUTOTUNE", "1") != "0"
-CTA_PAIR = os.environ.get("CB_GEMM_CTA_PAIR", "1") != "0"      # let the autotuner try the tcgen05 cta_group::2 kernel
-PAIR_SPLITK = os.environ.get("CB_GEMM_PAIR_SPLITK", "0") != "0"  # ... and its split-K form (measured: never wins, see DESIGN 4.1)
 # split-K slices as a thread-block cluster reducing through DSMEM (desc.splitk_cluster): an autotuner candidate on the lane-0
-# stream (=1, default), on every lane (=2) or never (=0).  History: with cluster launches on every stream the step hung against
-# the single-kernel GroupNorm that spun on a grid-wide counter; GroupNorm now runs on clusters too (no spinning kernel is left in
-# the bs=1 step) and both settings run clean (profiles/r02_ab_gn_cluster_and_cluster_splitk.jsonl); lane 0 stays the default
-# because a launch that falls back to the spinning GroupNorm is then ordered with the cluster GEMMs by the stream.
+# stream (=1, default), on every lane (=2) or never (=0).  Lane 0 is the default because a GroupNorm that falls back to the
+# single-kernel variant (CTAs spinning on a grid-wide counter) is then ordered with the cluster GEMMs by the stream; a pending
+# cluster and a half-resident spinning grid on concurrent streams could wait for each other.
 CLUSTER_SK = os.environ.get("CB_GEMM_CLUSTER_SK", "1") != "0"
 CLUSTER_SK_ALL_LANES = os.environ.get("CB_GEMM_CLUSTER_SK", "1") == "2"   # A/B aid: also beside concurrent streams
 # Front-end SM budget (CB_FE_CTAS = n > 0): the software-pipelined front end (VAE encode of the NEXT batch, lane 2) runs
-# its large GEMMs as persistent CTA-pair kernels on at most n CTAs and its streaming GroupNorm on at most n CTAs, so the
-# latency-bound chain of small launches that trains the CURRENT batch always finds free SMs instead of queueing behind a
-# wave of 8-10 us VAE CTAs (step_graph.py).  0 = every kernel sizes its grid for the whole device.
+# its large GEMMs as fixed 128 x (128 | 256) tiles without split-K (no autotuning) and its streaming GroupNorm on at most n
+# CTAs, so the latency-bound chain of small launches that trains the CURRENT batch finds free SMs instead of queueing behind
+# a wave of VAE CTAs (step_graph.py).  0 = every kernel sizes its grid for the whole device.
 FE_CTAS = int(os.environ.get("CB_FE_CTAS", "0"))
 FE_LANES = (2,)
 _TUNE = {}
@@ -118,40 +115,21 @@ def _autotune(d, key):
     M = d.img_n * d.out_h * d.out_w if d.conv else d.M
     taps = d.kh * d.kw if d.conv else 1
     kiters = taps * ((d.K + 63) // 64)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
     bns = [64] if d.N <= 64 else ([64, 128] if d.b_major == CB_MAJOR_MN else [64, 128, 160])
     if d.N >= 256 and d.a_major != CB_MAJOR_MN and M >= 1024 and os.environ.get("CB_GEMM_TILE256", "1") != "0":
         bns = bns + [256]          # 128x256 tiles (4-stage ring, one CTA per SM): fewer operand bytes per flop for large GEMMs
+    # Only knobs that leave the arithmetic unchanged are timed: tile width, ring depth and cluster vs workspace reduction
+    # of the k-slices.  The split count stays the library's (a function of the shape), so every
+    # candidate adds the same products in the same order and the winner of a noisy timing never changes the results.
     cands = [(0, 0, 0, 0, 0)]
     for bn in bns:
         tiles = ((d.N + bn - 1) // bn) * ((M + 127) // 128) * d.batch
-        cands.append((bn, 1, 0, 0, 0))
-        if tiles <= 148:
-            cands.append((bn, 1, 3, 0, 0))          # 3-stage ring: leaves room for the next kernel's CTAs on the SM
-        if tiles < 148:
-            for sp in (2, 3, 4, 6, 8, 12, 16, 24, 32):
-                if tiles * sp <= 320 and kiters // sp >= 2:
-                    cands.append((bn, sp, 0, 0, 0))
-                    if tiles * sp <= 148:
-                        cands.append((bn, sp, 3, 0, 0))
-                    if CLUSTER_SK and sp <= 16 and not d.glu:
-                        # the k-slices as one cluster, reduced through distributed shared memory; the exchange buffer
-                        # (slices x owned 8-column groups x 4 KiB) must fit the TMA ring the kernel will run with
-                        ring = 4 if bn == 256 else (6 if tiles * sp <= 148 else 3)
-                        if sp * (-(-(bn // 8) // sp)) * 4096 <= ring * (128 + bn) * 128:
-                            cands.append((bn, sp, 0, 0, 1))
-    if CTA_PAIR and d.a_major != CB_MAJOR_MN and M >= 2048 and d.N >= 128 and not d.d_transposed:
-        # tcgen05 cta_group::2: a 2-CTA cluster per 256 x bn tile (half the B bytes per SM); large-M GEMMs only
-        cands.append((128, 1, 0, 1, 0))
-        if d.N >= 256:
-            cands.append((256, 1, 0, 1, 0))
-    if CTA_PAIR and PAIR_SPLITK and d.a_major != CB_MAJOR_MN and 256 <= M <= 4096 and d.N >= 256 and not d.d_transposed \
-            and not d.glu and kiters >= 16:
-        # small-M / deep-K layers (16^2 / 32^2 convolutions, FF projections): 256 x 256 pair tiles halve the operand bytes
-        # every SM pulls out of L2 (the per-SM ingest limit is what bounds these launches), k-slices fill the SMs
-        ptiles = ((d.N + 255) // 256) * ((M + 255) // 256) * d.batch
-        for sp in (2, 3, 4, 6, 8, 12, 16, 24, 32):
-            if ptiles * sp <= 80 and kiters // sp >= 4:
-                cands.append((256, sp, 0, 1, 0))
+        cands.append((bn, 0, 0, 0, 0))
+        if tiles <= sms:
+            cands.append((bn, 0, 3, 0, 0))          # 3-stage ring: leaves room for the next kernel's CTAs on the SM
+        if CLUSTER_SK and not d.glu and kiters >= 8:
+            cands.append((bn, 0, 0, 0, 1))          # k-slices (if the library splits this shape) reduced inside a cluster
     t = GemmDesc.from_buffer_copy(bytes(d))
     # scratch output large enough for any addressing the descriptor can produce
     inner = d.batch_inner if d.batch_inner > 0 else d.batch

@@ -1,7 +1,7 @@
 """Deterministic synthetic checkpoints (there is no network for SD-v1 / CLIP / CosFace weights).
 
 Every tensor is drawn from a CPU generator seeded by (seed, sha1(key)), so a checkpoint is a pure function
-of its key names and shapes: the reference modules, the oracle restatement and the B200 engines all see
+of its key names and shapes: the reference modules, the oracle restatement and the H100 engines all see
 bit-identical fp32 weights without shipping gigabytes.  Rules (SURVEY.md §8c "synthetic-weight rules"):
 variance-preserving fan-in init for every matrix/conv (including the reference's zero-initialised
 modules, which would otherwise make every output and gradient exactly 0, and iresnet convs, whose own

@@ -1,4 +1,4 @@
-"""One CelebBasis training step (SURVEY.md §8 rows a1-a31) on the sm_100a kernels.
+"""One CelebBasis training step (SURVEY.md §8 rows a1-a31) on the sm_90a kernels.
 
     image --VAE encode--> z --q_sample(t, noise)--> x_t --\
     faces --warp/resize--> CosFace R100 --> v -- MLP(W,b) --> coef --basis--> 2 token embeddings      UNet --> eps

@@ -1,4 +1,4 @@
-"""SD-v1 UNet forward + activation-gradient backward on the sm_100a kernels.
+"""SD-v1 UNet forward + activation-gradient backward on the sm_90a kernels.
 
 This is the executor behind ldm.modules.diffusionmodules.openaimodel.UNetModel in the host mirror.
 It follows the reference's module graph exactly (openaimodel.py:413-742 UNetModel, :163-275 ResBlock,
@@ -6,7 +6,7 @@ It follows the reference's module graph exactly (openaimodel.py:413-742 UNetMode
 but runs it as an explicit tape of kernel launches:
 
   * activations are channels-last matrices [N*H*W][C]; the residual stream, norm inputs and block
-    outputs stay fp32, every tensor-core operand is fp16 (or bf16), accumulation is fp32 in TMEM;
+    outputs stay fp32, every tensor-core operand is fp16 (or bf16), accumulation is fp32 in registers;
   * all 22 ResBlock `emb_layers` linears are one GEMM per step whose output slice is the per-image
     bias of that block's first conv (fused in the conv epilogue together with the conv bias);
   * q/k/v (self) and k/v (cross) projections are single GEMMs over concatenated weights;
@@ -30,8 +30,8 @@ class _Attn:
     """softmax(q k^T * scale) v for (image, head) batches.  What is kept for the backward pass is either the
     log-sum-exp + output (flash backward, nothing quadratic in HBM) or the probabilities (materialised path)."""
 
-    FLASH = True       # fused tcgen05 flash kernel for head dims <= 128 (set False to force the materialised path)
-    FLASH_BWD = True   # recompute-in-TMEM backward (cb_attention_bwd) instead of P / dP / dS round trips through HBM
+    FLASH = True       # fused wgmma flash kernel for head dims <= 128 (set False to force the materialised path)
+    FLASH_BWD = True   # recompute-in-registers backward (cb_attention_bwd) instead of P / dP / dS round trips through HBM
     FLASH_BWD_MIN_NK = 256   # short key sequences (cross attention on 77 tokens): the materialised path has more CTAs
 
     @staticmethod
@@ -44,7 +44,7 @@ class _Attn:
                                            causal=causal, want_lse=True)
                 return ("lse", lse, out, causal)
             if need_p and _Attn.FLASH_BWD:
-                # short key sequence (cross attention): keep P and lse; the backward rebuilds dS in TMEM (dQ kernel) and
+                # short key sequence (cross attention): keep P and lse; the backward rebuilds dS in registers (dQ kernel) and
                 # exports it, dK / dV are two small GEMMs over P and dS
                 P, lse = ops.attention_fwd(q, k, v, out, images=images, heads=heads, dh=dh, nq=nq, nk=nk, scale=scale,
                                            causal=causal, want_p=True, want_lse=True)

@@ -1,4 +1,4 @@
-"""AutoencoderKL.encode (first-stage encoder + quant_conv) on the sm_100a kernels, forward only / no grad.
+"""AutoencoderKL.encode (first-stage encoder + quant_conv) on the sm_90a kernels, forward only / no grad.
 
 Mirrors ldm/models/autoencoder.py:324-328 -> ldm/modules/diffusionmodules/model.py:434-459 (Encoder.forward),
 :82-141 (ResnetBlock), :150-202 (AttnBlock: 1 head over all pixels), :60-79 (Downsample: pad (0,1,0,1) + stride 2).

@@ -1,5 +1,5 @@
 /*
- * celebbasis_b200 — C-ABI of the B200-native (sm_100a) hot path of CelebBasis.
+ * celebbasis_b200 — C-ABI of the H100-native (sm_90a) hot path of CelebBasis.
  *
  * The reference (ygtxr1997/CelebBasis) has no FFI: its hot path is a chain of stock ATen calls
  * made from Python (SURVEY.md §8b).  This header is therefore the boundary a maintainer would
@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CB_ABI_VERSION 4
+#define CB_ABI_VERSION 5
 #define CB_GN_WS_BYTES 131072
 
 /* element types */
@@ -42,7 +42,7 @@ enum {
     CB_ERR_ARG = -1,       /* invalid argument / unsupported shape */
     CB_ERR_ALIGN = -2,     /* pointer or stride alignment */
     CB_ERR_DRIVER = -3,    /* CUDA driver entry point unavailable / tensor-map encode failed */
-    CB_ERR_NO_DEVICE = -4, /* no sm_100 device */
+    CB_ERR_NO_DEVICE = -4, /* no sm_90 device */
 };
 
 int cb_abi_version(void);
@@ -53,7 +53,7 @@ int cb_device_ok(void);
 unsigned long long cb_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * cb_gemm — tcgen05 tensor-core GEMM / implicit-GEMM convolution with TMA-staged operands.
+ * cb_gemm — wgmma tensor-core GEMM / implicit-GEMM convolution with TMA-staged operands.
  *
  *   D[b][m][n] = act(alpha * sum_{tap,k} A_tap[b][m][k] * B[b][tap][n][k] + bias[...]) + R[b][m][n]
  *
@@ -126,11 +126,12 @@ typedef struct cb_gemm_desc {
     int32_t batch_inner;
     int64_t a_batch_stride2, b_batch_stride2, d_batch_stride2, r_batch_stride2;
 
-    /* optional split-K workspace (caller-owned, 64 KiB of counters + one fp32 accumulator tile per output tile; it
-     * must be ALL ZERO before its first use and every launch leaves it all zero).  With it, shapes whose tile grid
-     * cannot fill the SMs (bs=1 low-resolution layers: M <= 256 rows against 1280-2560 channel weights) spread
-     * their k-loop over several CTAs that red.global.add their fp32 partial tiles into the accumulator; the last
-     * CTA of a tile runs the epilogue.  NULL disables split-K.  Launches sharing a workspace must be stream-ordered. */
+    /* optional split-K workspace (caller-owned, 64 KiB of counters + one fp32 partial tile per k-slice and output
+     * tile; the counters must be ALL ZERO before its first use and every launch leaves them zero).  With it, shapes
+     * whose tile grid cannot fill the SMs (bs=1 low-resolution layers: M <= 256 rows against 1280-2560 channel
+     * weights) spread their k-loop over several CTAs that store their fp32 partial tiles into their own slices; the
+     * last CTA of a tile adds them in slice order (bit-reproducible) and runs the epilogue.  NULL disables split-K.
+     * Launches sharing a workspace must be stream-ordered. */
     void* splitk_ws;
     int64_t splitk_ws_bytes;
 
@@ -139,16 +140,15 @@ typedef struct cb_gemm_desc {
     void* debug_timeline;
 
     /* tuning overrides, 0 = the library's cost model: tile width (64 / 128 / 160 / 256; 160 only with K-major B) and the
-     * number of split-K slices (1 = no split; ignored when the workspace cannot hold it).  The host autotuner
-     * (celebbasis_b200/ops.py) times the candidates once per shape and passes the winner here. */
+     * number of split-K slices (1 = no split; ignored when the workspace cannot hold it).  Without a splits request
+     * the split count depends on the shape only, never on tile_n / stages / cta_pair / splitk_cluster, so those knobs
+     * do not change the results.  The host autotuner (celebbasis_b200/ops.py) times them once per shape and passes the
+     * winner here. */
     int32_t tile_n;
     int32_t splits;
     int32_t stages;      /* 0 = auto, 3 = 3-stage ring / 2 CTAs per SM, 6 = 6-stage ring / 1 CTA per SM */
-    int32_t cta_pair;    /* >= 1 = tcgen05 cta_group::2 variant: a 2-CTA cluster computes a 256 x (128|256) tile, each CTA
-                          * staging its 128 rows of A and half of the B tile (K-major A; `splits` > 1 spreads the k-slices of
-                          * a tile over clusters); the kernel is persistent on min(work items, SMs / 2) clusters, or on at
-                          * most n CTAs when cta_pair = n >= 2 (a throughput-bound producer that shares the device with a
-                          * latency-bound chain leaves the other SMs to it); 0 = single-CTA tiles */
+    int32_t cta_pair;    /* tile request of the host autotuner: >= 1 = large-M tiles (128 x 128 or 128 x 256 by tile_n;
+                          * sm_90 has no two-CTA MMA, so every tile is one CTA); 0 = the library's choice */
 
     /* second destination (optional, batch == 1, not transposed): the same epilogue value is also written to
      * D2[row][col] (row pitch ldd2 elements, dtype d2_dtype).  Used to place a UNet skip activation straight into the
@@ -179,8 +179,8 @@ int cb_gemm(const cb_gemm_desc* desc, void* stream);
 
 
 /* ---------------------------------------------------------------------------------------------
- * Normalisation (channels-last).  ws = caller workspace of CB_GN_WS_BYTES bytes (group sums or per-CTA partial
- * slots, plus a self-resetting grid arrival counter in its last 8 bytes); the caller zeroes it ONCE at allocation;
+ * Normalisation (channels-last).  ws = caller workspace of CB_GN_WS_BYTES bytes (per-CTA partial sums, added up in
+ * CTA order, plus a self-resetting grid arrival counter in its last 8 bytes); the caller zeroes it ONCE at allocation;
  * calls sharing it must be stream-ordered.
  * cb_groupnorm_*: ldm/modules/diffusionmodules/util.py:199-216 (GroupNorm32, eps 1e-5),
  *   ldm/modules/attention.py:76-77 and ldm/modules/diffusionmodules/model.py:38-39 (Normalize, eps 1e-6),
@@ -316,8 +316,8 @@ int cb_ema_rows(float* table, const long long* idx, int idx_stride, const float*
                 float momentum, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * cb_attention_fwd -- fused softmax(Q K^T * scale [+ causal mask]) V on tcgen05 (flash style): the scores live in
- * TMEM, K/V blocks of 128 keys are TMA-staged in shared memory, the softmax is one thread per query row.
+ * cb_attention_fwd -- fused softmax(Q K^T * scale [+ causal mask]) V with wgmma (flash style): the scores live in
+ * registers, K/V blocks of 64 keys are TMA-staged in shared memory, the softmax runs on the accumulator fragments.
  * Replaces ldm/modules/attention.py:178-191 (CrossAttention: self and cross) and the masked CLIP attention driven
  * from ldm/modules/encoders/modules.py:24-31,320-340.
  *   Q [images*nq][ldq], K/V [images*nk][ldk/ldv], O [images*nq][ldo]: head h occupies columns [h*d, (h+1)*d);
@@ -334,7 +334,7 @@ int cb_attention_fwd(const void* Q, long long ldq, const void* K, long long ldk,
 /* ---------------------------------------------------------------------------------------------
  * cb_attention_bwd -- flash-style backward of the same attention (the gradient torch.autograd derives for
  * ldm/modules/attention.py:178-191): dQ, dK, dV from Q, K, V, O, dO and the forward's lse, recomputing the
- * probabilities tile by tile in TMEM; no (heads x N x N) tensor and no atomics.  Two launches: query-stationary
+ * probabilities tile by tile in registers; no (heads x N x N) tensor and no atomics.  Two launches: query-stationary
  * (dQ, also writes delta = rowsum(dO o O)) then key-stationary (dK, dV).
  *   layouts as cb_attention_fwd; dQ/dK/dV use the layouts of Q/K/V with their own row pitches;
  *   delta: caller workspace [images][heads][nq] fp32.

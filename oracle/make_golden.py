@@ -90,7 +90,7 @@ def run(kind):
         "momentum": float(model.embedding_manager.momentum),
     }
     if kind == "tiny":
-        out["gW"] = W.grad.detach().clone()
+        out["gW_rows8"] = W.grad.detach()[::8].clone()       # every 8th output row: the file stays under 1 MB
         out["face_in"] = cap["face_in"]
     else:
         out["gW_sample"] = W.grad.detach().flatten()[::131].clone()
@@ -151,7 +151,8 @@ def run_infer(kind="tiny", steps=4, scale=5.0):
            "uc": uc.clone(), "c": c.clone(), "x_T": x_T.clone(), "samples": samples.clone(), "img": img.clone(),
            "ddim_timesteps": torch.as_tensor(np.asarray(sampler.ddim_timesteps).copy())}
     os.makedirs(GOLD, exist_ok=True)
-    torch.save(out, os.path.join(GOLD, f"infer_{kind}.pt"))
+    # non-zip serialization: no per-record zip padding, which keeps the file under 10^6 bytes
+    torch.save(out, os.path.join(GOLD, f"infer_{kind}.pt"), _use_new_zipfile_serialization=False)
     print(f"[infer/{kind}] samples |x|={samples.norm().item():.6f} img |x|={img.norm().item():.6f} "
           f"timesteps={out['ddim_timesteps'].tolist()}")
 
@@ -184,7 +185,8 @@ def run_curve(kind="tiny", steps=50, lr=5e-3):
         ts.append(int(draws["t"][0]))
     lin = em.meta_id_net.stylegan_mlp.net[0]
     out = {"kind": kind, "steps": steps, "lr": lr, "losses": torch.tensor(losses, dtype=torch.float64), "t": ts,
-           "W_final": lin.weight.detach().clone(), "b_final": lin.bias.detach().clone(),
+           "W_final_rows4": lin.weight.detach()[::4].clone(),   # every 4th output row
+           "b_final": lin.bias.detach().clone(),
            "ema_coef_id0_init": init["coef"], "ema_emb_id0_init": init["emb"],
            "ema_coef_id0": em.id_coefficients[0].detach().clone(), "ema_emb_id0": em.id_embeddings[0].detach().clone(),
            "optimizer": type(opt).__name__, "opt_defaults": {k: v for k, v in opt.defaults.items() if isinstance(v, (int, float, tuple, bool))}}
@@ -264,7 +266,9 @@ def run_ti():
             em.save(os.path.join(td, "ti.pt"))
             ck = torch.load(os.path.join(td, "ti.pt"), weights_only=False)
         cases.append({"nv": nv, "ids": ids, "text_seed": 5, "text_sum": float(text.double().sum()),
-                      "out": out.detach().clone(), "ids_after": ids_in.clone(),
+                      # only the rows of `out` that differ from the seeded input text (the rest is that text)
+                      "out_rows": (out.detach() != text).any(-1).nonzero(),
+                      "out_vals": out.detach()[(out.detach() != text).any(-1)].clone(), "ids_after": ids_in.clone(),
                       "params": {k: v.detach().clone() for k, v in em.string_to_param_dict.items()},
                       "tokens": {k: int(v) for k, v in em.string_to_token_dict.items()},
                       "grads": {k: (v.grad.detach().clone() if v.grad is not None else None)
@@ -300,7 +304,7 @@ def run_data():
                                                  np.random.get_state()[2], torch.get_rng_state().numpy().tobytes()))).hexdigest()
                 items.append({"split": split, "diff_cnt": diff, "index": i, "caption": ex["caption"],
                               "ids": ex["image_ori"]["ids"].clone(), "num_ids": ex["image_ori"]["num_ids"],
-                              "image": ex["image"].clone(), "faces": ex["image_ori"]["faces"].clone(), "rng_digest": dig,
+                              "image": ex["image"].half(), "faces": ex["image_ori"]["faces"].half(), "rng_digest": dig,
                               "len": len(ds)})
     torch.save({"hw": hw, "items": items, "seed": 11}, os.path.join(GOLD, "data_path.pt"))
     print("[data]", [(it["index"], it["caption"], it["ids"].tolist()) for it in items])

@@ -19,7 +19,7 @@ def test_library_loads_and_exports_header_symbols():
     assert len(syms) >= 35
     for s in syms:
         assert hasattr(L, s), f"symbol {s} declared in the header but not exported"
-    assert L.cb_abi_version() == 4
+    assert L.cb_abi_version() == 5
     assert isinstance(lib.last_error(), str)
 
 
@@ -49,7 +49,7 @@ def test_gemm_desc_layout_matches_header():
 
 
 def test_no_cpu_fallback_without_device():
-    """Without an sm_100 device the product path must fail loudly (no oracle / CPU fallback)."""
+    """Without an sm_90 device the product path must fail loudly (no oracle / CPU fallback)."""
     import pytest
     import torch
     if torch.cuda.is_available():
@@ -62,6 +62,6 @@ def test_no_cpu_fallback_without_device():
 
 
 def test_graft_entry_build():
-    """The driver's build hook: compiles (cached) every CUDA source for sm_100a, loads the library, checks the ABI."""
+    """The driver's build hook: compiles (cached) every CUDA source for sm_90a, loads the library, checks the ABI."""
     import __graft_entry__ as g
     g.build()

@@ -19,7 +19,7 @@ def dev():
     if not torch.cuda.is_available():
         pytest.skip("needs a GPU")
     from celebbasis_b200 import lib
-    assert lib.load().cb_device_ok() == 1, "tests must run on an sm_100 device"
+    assert lib.load().cb_device_ok() == 1, "tests must run on an sm_90 device"
     return torch.device("cuda:0")
 
 
@@ -106,7 +106,7 @@ def test_conv_stride2_dgrad_via_zero_insertion(dev):
 @pytest.mark.parametrize("nq,nk,dh,heads,images", [(1024, 1024, 40, 8, 1), (256, 77, 160, 8, 2), (77, 77, 64, 12, 2),
                                                    (64, 64, 160, 8, 1)])
 def test_attention_fwd_bwd(dev, nq, nk, dh, heads, images):
-    """q.k^T softmax p.v as batched tcgen05 GEMMs (K-major and MN-major operands), forward and backward."""
+    """q.k^T softmax p.v as batched wgmma GEMMs (K-major and MN-major operands), forward and backward."""
     from celebbasis_b200.unet_engine import _Attn
     C = heads * dh
     q, k, v = rnd(images * nq, C), rnd(images * nk, C), rnd(images * nk, C)
@@ -300,7 +300,7 @@ def test_face_warp_resize(dev):
                                                           (300, 200, 128, 2, 1, False), (64, 64, 40, 8, 1, False),
                                                           (200, 330, 40, 2, 2, True)])
 def test_flash_attention_bwd(dev, nq, nk, dh, heads, images, causal):
-    """cb_attention_bwd (P, dP, dS rebuilt tile by tile in TMEM from the forward's log-sum-exp; dQ then dK/dV, no
+    """cb_attention_bwd (P, dP, dS rebuilt tile by tile in registers from the forward's log-sum-exp; dQ then dK/dV, no
     atomics) vs torch.autograd of softmax(QK^T*scale)V in fp32 on the same fp16 inputs."""
     from celebbasis_b200 import ops
     C = heads * dh
@@ -347,7 +347,7 @@ def test_flash_attention_bwd(dev, nq, nk, dh, heads, images, causal):
                                                           (64, 64, 40, 8, 1, False)])
 @pytest.mark.parametrize("want_p", [False, True])
 def test_flash_attention_fwd(dev, nq, nk, dh, heads, images, causal, want_p):
-    """cb_attention_fwd (scores in TMEM, online softmax, P.V in TMEM) vs softmax(QK^T*scale)V in fp32; one-pass
+    """cb_attention_fwd (scores in registers, online softmax, P.V in registers) vs softmax(QK^T*scale)V in fp32; one-pass
     (inference) and two-pass (probabilities exported for the backward) modes."""
     from celebbasis_b200 import ops
     C = heads * dh
@@ -479,7 +479,7 @@ def test_ema_rows_and_prep_kernels(dev):
 
 @pytest.mark.parametrize("bn", [128, 256])
 def test_gemm_cta_pair(dev, bn):
-    """tcgen05 cta_group::2 variant (desc.cta_pair = 1): a 2-CTA cluster per 256 x bn tile.  Linear K-major / MN-major B,
+    """desc.cta_pair = 1 requests (single-CTA 128 x bn tiles on sm_90).  Linear K-major / MN-major B,
     3x3 convolution (padding, ragged rows), odd tile counts, bias + residual + second destination."""
     from celebbasis_b200 import ops
     orig = ops._gemm
@@ -518,9 +518,8 @@ def test_gemm_cta_pair(dev, bn):
 
 @pytest.mark.parametrize("splits,cap", [(2, 1), (5, 1), (12, 1), (3, 16)])
 def test_gemm_cta_pair_splitk(dev, splits, cap):
-    """Split-K inside the CTA-pair kernel (desc.cta_pair >= 1, desc.splits > 1): the k-slices of a 256 x 256 tile run on
-    different clusters and meet in the L2 workspace (one tile + counter per CTA of a pair); desc.cta_pair = n >= 2 caps the
-    persistent grid at n CTAs.  Small-M / deep-K shapes of the 16^2 / 32^2 UNet levels, ragged M / N, odd tile counts,
+    """Split-K with pair tile requests (desc.cta_pair >= 1, desc.splits > 1): the k-slices of a 128 x 256 tile meet in the
+    L2 workspace.  Small-M / deep-K shapes of the 16^2 / 32^2 UNet levels, ragged M / N, odd tile counts,
     bias + residual, MN-major B, repeated launches (the workspace must come back zeroed)."""
     from celebbasis_b200 import ops
     orig = ops._gemm
@@ -621,8 +620,7 @@ def test_gemm_cluster_splitk(dev, bn, splits):
 
 
 def test_front_end_sm_budget(dev):
-    """ops.FE_CTAS (env CB_FE_CTAS): inside the front-end lane the large GEMMs run as persistent CTA-pair kernels on at
-    most n CTAs (stride-2 / asymmetric padding of the VAE downsample included) and the streaming GroupNorm pair on at
+    """ops.FE_CTAS (env CB_FE_CTAS): inside the front-end lane the large GEMMs run as pair tile requests (stride-2 / asymmetric padding of the VAE downsample included) and the streaming GroupNorm pair on at
     most n CTAs; results are unchanged."""
     from celebbasis_b200 import ops
     old = ops.FE_CTAS

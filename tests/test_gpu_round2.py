@@ -101,12 +101,13 @@ def test_mlp_gradient_elementwise_outside_leakyrelu_flips(dev, golden_dir):
     pre_our = eng.last["face_feat"].float().cpu() @ W.t() + bias
     flipped = ((pre_ref > 0) != (pre_our > 0)).any(0)               # output neurons with a sign flip in any face row
     same = ~flipped
-    gW, gWr = eng.gW.float().cpu(), gold["gW"].float()
     gb, gbr = eng.gb.float().cpu(), gold["gb"].float()
     n_flip = int(flipped.sum())
     assert n_flip <= 0.02 * flipped.numel(), n_flip
-    assert rel(gW[same], gWr[same]) < 1e-2, rel(gW[same], gWr[same])
     assert rel(gb[same], gbr[same]) < 1e-2
+    # the stored reference gradient holds every 8th output row
+    gW, gWr, same = eng.gW.float().cpu()[::8], gold["gW_rows8"].float(), same[::8]
+    assert rel(gW[same], gWr[same]) < 1e-2, rel(gW[same], gWr[same])
     # element-wise: >97% of the elements of the agreeing rows within 2e-2 of the row scale
     scale = gWr[same].abs().mean(1, keepdim=True) + 1e-30
     frac_ok = ((gW[same] - gWr[same]).abs() <= 2e-2 * scale * 10).float().mean().item()
@@ -140,8 +141,8 @@ def test_loss_curve_50_steps_vs_reference_golden(dev, golden_dir):
     assert rel(eng.id_embeddings[0], gold["ema_emb_id0"]) <= 1e-2
     # the trained weights: AdamW moves every element by ~lr per step whatever the gradient's size, so elements whose
     # gradient is round-off sized can walk apart; the bulk must agree
-    dW_ref = gold["W_final"] - eng_initial_W(gold, golden_dir)
-    dW = eng.W.cpu() - eng_initial_W(gold, golden_dir)
+    dW_ref = gold["W_final_rows4"] - eng_initial_W(gold, golden_dir)[::4]       # every 4th output row is stored
+    dW = eng.W.cpu()[::4] - eng_initial_W(gold, golden_dir)[::4]
     assert cos(dW, dW_ref) > 0.98, cos(dW, dW_ref)
 
 
@@ -218,10 +219,7 @@ def test_batch2_step_equals_mean_of_single_steps(dev):
 
 def test_step_graphs_pipelined_equals_serial(dev):
     """The software pipeline only changes WHEN a batch's frozen front end runs: losses / gradients / latents of the
-    pipelined schedule must equal the serial schedule's up to the engine's run-to-run noise.  (The engine is not bitwise
-    reproducible: split-K partial tiles are reduced with red.global.add.f32 and GroupNorm sums with fp64 atomics, so
-    the summation order varies; per launch that is 1e-8 (fp32 outputs) / one fp16 rounding flip in 1e5 elements, and
-    through the 100-layer CosFace net it grows to ~1.5e-3 on v -- tools/diag_determinism.py, tools/diag_pipe.py.)"""
+    pipelined schedule must equal the serial schedule's (the front end runs on other streams, beside the chain)."""
     from celebbasis_b200 import workload
     from celebbasis_b200.step_graph import StepGraphs
     eng, _, _ = _engine("tiny", dev)
@@ -265,6 +263,24 @@ def test_step_graphs_pipelined_equals_serial(dev):
     b, d = _to_dev(stream[1][0], stream[1][1], dev)
     loss_e = eng.forward_backward(b, d, ema_update=False).item()
     assert abs(loss_e - ser[1][0]) / abs(loss_e) < 1e-3
+
+
+def test_step_is_bit_reproducible(dev):
+    """Every reduction of the training step adds in a fixed order (split-K slices, GroupNorm partials, the loss, the
+    inject backward), so the same step on the same inputs gives bit-identical loss, gradient and predicted noise -- the
+    property that keeps two training runs (and two benchmark runs) from drifting apart under AdamW."""
+    from celebbasis_b200 import workload
+    eng, _, _ = _engine("tiny", dev)
+    batch, draws = workload.synth_batch("tiny", B=1, seed=1234)
+    b, d = _to_dev(batch, draws, dev)
+    outs = []
+    for _ in range(3):
+        loss = eng.forward_backward(b, d, ema_update=False)
+        torch.cuda.synchronize()
+        outs.append((loss.detach().clone(), eng.grad.clone(), eng.last["eps"].clone(), eng.last["context"].clone()))
+    for o in outs[1:]:
+        for x, y in zip(outs[0], o):
+            assert torch.equal(x, y)
 
 
 def test_trainer_fit_fused_api_equals_eager_modules(dev):
@@ -433,7 +449,9 @@ def test_textual_inversion_manager_vs_reference_golden(dev, golden_dir):
         text = torch.randn(len(gold["prompts"]), 77, 768, generator=g).to(dev)
         ids = case["ids"].clone().to(dev)
         out = em(ids, text)
-        assert torch.equal(out.cpu(), case["out"]), nv
+        exp = torch.randn(len(gold["prompts"]), 77, 768, generator=torch.Generator().manual_seed(case["text_seed"]))
+        exp[case["out_rows"][:, 0], case["out_rows"][:, 1]] = case["out_vals"]      # rows the manager rewrote
+        assert torch.equal(out.cpu(), exp), nv
         if nv > 1:
             assert torch.equal(ids.cpu(), case["ids_after"])
         out.sum().backward()

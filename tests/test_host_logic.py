@@ -248,7 +248,7 @@ def test_groupnorm_cluster_plan_covers_the_step():
                 continue
             S, gpc, rows, smem = p
             cpg, cw = c // 32, gpc * (c // 32)
-            assert S * (32 // gpc) <= 148 and S * rows >= hw and S <= 16 and 32 % gpc == 0
+            assert S * (32 // gpc) <= 132 and S * rows >= hw and S <= 16 and 32 % gpc == 0
             assert rows * cw * bpe <= smem <= 200 * 1024 and cw % 4 == 0
             # the kernels' thread map on one CTA: quad cq = tid % nq, row lane ry = tid // nq, RY = 512 // nq row lanes
             nq = cw // 4
@@ -375,7 +375,9 @@ def test_textual_inversion_row_map_vs_reference(golden_dir):
         for b in range(text.shape[0]):
             for i in range(77):
                 out[b, i] = text[b, m[b, i]] if m[b, i] >= 0 else zr[-(m[b, i] + 1)]
-        assert torch.equal(out, case["out"]), nv
+        exp = torch.randn(len(gold["prompts"]), 77, 768, generator=torch.Generator().manual_seed(case["text_seed"]))
+        exp[case["out_rows"][:, 0], case["out_rows"][:, 1]] = case["out_vals"]      # rows the manager rewrote
+        assert torch.equal(out, exp), nv
         if nv > 1:
             assert torch.equal(torch.from_numpy(new_tok), case["ids_after"])
         assert case["ckpt_keys"] == ["string_to_param", "string_to_token"]

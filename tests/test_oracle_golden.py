@@ -59,7 +59,7 @@ def test_tiny_step_matches_reference(golden_dir):
     assert _rel(out["x_noisy"], gold["x_noisy"]) < 1e-5
     assert _rel(out["eps"], gold["eps"]) < 1e-4
     assert abs(out["loss"].item() - gold["loss"].item()) / abs(gold["loss"].item()) < 1e-5
-    assert _rel(W.grad, gold["gW"]) < 1e-3
+    assert _rel(W.grad[::8], gold["gW_rows8"]) < 1e-3 and abs(W.grad.norm().item() / gold["gW_norm"].item() - 1) < 1e-3
     assert _rel(b.grad, gold["gb"]) < 1e-3
     assert gold["graded"] == ["embedding_manager.meta_id_net.stylegan_mlp.net.0.weight",
                               "embedding_manager.meta_id_net.stylegan_mlp.net.0.bias"]

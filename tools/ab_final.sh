@@ -1,8 +1,8 @@
 #!/bin/bash
 # A/B of the cluster GroupNorm (default on) and the cluster split-K variants on one box; every leg under its own hard timeout
-# (a hung leg must not take the rest of the call with it).  Outputs under gpurun_out/.
+# (a hung leg must not take the rest of the call with it).  Outputs under tools_out/.
 T=${1:-r02e}
-O=gpurun_out
+O=tools_out
 timeout -s KILL 330 python -m pytest tests -x -q -m gpu > $O/${T}_pytest_gpu.log 2>&1; tail -3 $O/${T}_pytest_gpu.log
 run() {   # name, env assignments...
     local name=$1; shift

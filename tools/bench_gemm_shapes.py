@@ -11,7 +11,7 @@ from celebbasis_b200 import ops
 
 dev = torch.device("cuda:0")
 g = torch.Generator().manual_seed(0)
-out_path = os.path.join(ROOT, "gpurun_out", "gemm_shapes.jsonl")
+out_path = os.path.join(ROOT, "tools_out", "gemm_shapes.jsonl")
 os.makedirs(os.path.dirname(out_path), exist_ok=True)
 
 

@@ -70,7 +70,7 @@ for key, items in groups.items():
 rows.sort(key=lambda r: -r["total_us"])
 tot = sum(r["total_us"] for r in rows); totf = sum(r["gflop"] * r["count"] for r in rows)
 print(f"# {len(rec)} GEMMs, {len(rows)} shapes, sum of isolated times {tot/1000:.2f} ms, {totf:.0f} GFLOP -> {totf/tot*1e3/1e3:.1f} TFLOP/s")
-out = os.path.join(ROOT, "gpurun_out", "gemm_breakdown.jsonl")
+out = os.path.join(ROOT, "tools_out", "gemm_breakdown.jsonl")
 with open(out, "w") as f:
     for r in rows:
         f.write(json.dumps(r) + "\n")

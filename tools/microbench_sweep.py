@@ -1,5 +1,5 @@
 """BASELINE config 5: attention / conv microbench sweep with both roofline fractions per row (SURVEY 8d definitions:
-algorithmic FLOPs and bytes, recompute not counted; peaks from MEASURED_PEAKS.json).  One JSON line per case."""
+algorithmic FLOPs and bytes, recompute not counted; peaks from the H100 SXM data sheet).  One JSON line per case."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -9,12 +9,8 @@ from celebbasis_b200.unet_engine import _Attn
 dev = torch.device("cuda:0")
 g = torch.Generator().manual_seed(0)
 rnd = lambda *s: torch.randn(*s, generator=g).half().to(dev)
-try:
-    pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-except Exception:
-    pk = {}
-PEAK_TF, PEAK_GB = float(pk.get("bf16_tflops_sustained", 1451.1)), float(pk.get("hbm_gbs", 6586.1))
-out_path = os.path.join(ROOT, "gpurun_out", "microbench_sweep.jsonl")
+PEAK_TF, PEAK_GB = 989.0, 3350.0      # H100 SXM data sheet, dense BF16 / HBM3 (700 W); never reached
+out_path = os.path.join(ROOT, "tools_out", "microbench_sweep.jsonl")
 os.makedirs(os.path.dirname(out_path), exist_ok=True)
 open(out_path, "w").close()
 

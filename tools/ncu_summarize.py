@@ -4,7 +4,7 @@
   profiles/r02_gemm_traffic.json       DRAM bytes per cb_gemm launch + the sha1 of cb_gemm.cu they were measured on
                                        (bench.py reports roofline.traffic only while that sha1 matches the source tree)
 
-    python tools/ncu_summarize.py gpurun_out/r02_step_metrics_ncu.csv
+    python tools/ncu_summarize.py tools_out/r02_step_metrics_ncu.csv
 """
 import collections
 import csv

@@ -2,7 +2,7 @@
 
 Run on the GPU box:  python tools/probe_gemm.py [group ...]
 Each group runs in its own subprocess so a device trap in one group does not mask the others.
-Results: gpurun_out/gemm_probe.jsonl
+Results: tools_out/gemm_probe.jsonl
 """
 import json
 import os
@@ -12,7 +12,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-OUT = os.path.join(ROOT, "gpurun_out")
+OUT = os.path.join(ROOT, "tools_out")
 os.makedirs(OUT, exist_ok=True)
 
 GROUPS = ["basic", "mn", "conv", "conv_s2", "dgrad", "timing"]

@@ -6,7 +6,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-OUT = os.path.join(ROOT, "gpurun_out")
+OUT = os.path.join(ROOT, "tools_out")
 os.makedirs(OUT, exist_ok=True)
 
 import torch

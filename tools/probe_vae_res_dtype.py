@@ -1,5 +1,4 @@
-"""Probe: VAE encoder with an fp32 vs fp16 residual stream -- latent parity against the reference fixture and time.
-(Result on B200: fp32 z rel 5.9e-4 / 2.91 ms; fp16 z rel 7.3e-4 / 2.71 ms: not worth the parity budget.)"""
+"""Probe: VAE encoder with an fp32 vs fp16 residual stream -- latent parity against the reference fixture and time."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

@@ -1,5 +1,5 @@
-"""Opcode histogram per kernel of libcelebbasis_b200.so (cuobjdump -sass): the Blackwell-native evidence
-(UTCHMMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk, SYNCS = mbarrier;
+"""Opcode histogram per kernel of libcelebbasis_b200.so (cuobjdump -sass): which tensor-core and copy paths each kernel uses
+(HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, UBLKCP = cp.async.bulk, SYNCS = mbarrier;
 HMMA would be the legacy mma.sync path).  Writes profiles/sass_summary.txt.
 
     python tools/sass_summary.py
@@ -12,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "celebbasis_b200", "libcelebbasis_b200.so")
-KEY = ["UTCHMMA", "UTCQMMA", "UTCOMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UTCBAR", "UTCATOM",
+KEY = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "SYNCS", "UTCBAR", "UTCATOM",
        "HMMA", "IMMA", "MUFU", "REDG", "RED", "ATOMG", "ATOM", "LDG", "STG", "LDS", "STS", "BAR", "ACQBULK", "ELECT"]
 
 
@@ -38,10 +38,10 @@ def main():
         short = short.replace("void ", "")
         hot = " ".join(f"{k}={cnt[k]}" for k in KEY if cnt.get(k))
         lines.append(f"{short[:110]:110s} instr={sum(cnt.values()):6d}  {hot}")
-    hdr = [f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}  ({len(per)} kernels, sm_100a)",
+    hdr = [f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}  ({len(per)} kernels, sm_90a)",
            "# totals: " + " ".join(f"{k}={total[k]}" for k in KEY if total.get(k)),
-           "# tcgen05/TMA proof: UTCHMMA (tcgen05.mma kind::f16), LDTM/STTM (tcgen05.ld/st), UTMALDG (cp.async.bulk.tensor), "
-           "UBLKCP (cp.async.bulk), SYNCS (mbarrier); HMMA (legacy mma.sync) must be absent", ""]
+           "# HGMMA (wgmma.mma_async), UTMALDG (cp.async.bulk.tensor), UBLKCP (cp.async.bulk), SYNCS (mbarrier); "
+           "HMMA (legacy mma.sync) must be absent", ""]
     text = "\n".join(hdr + sorted(lines)) + "\n"
     dst = os.path.join(ROOT, "profiles", "sass_summary.txt")
     with open(dst, "w") as f:
