@@ -62,7 +62,6 @@ struct GemmParams {
     float* ws;
     unsigned* counters;
     int cluster_sk;           // split-K through distributed shared memory: the `splits` CTAs of a tile form a cluster (1,1,splits)
-    int ws_tr;                // accumulator-tile layout in ws: 1 = float4-group-major (coalesced warp requests), 0 = row-major
     int dbg_mode;             // tuning aid (env CB_GEMM_DBG_MODE): 1 exit after setup, 2 skip epilogue, 3 exit at once
     unsigned long long* dbg;  // optional per-CTA timeline (8 x u64 globaltimer ns per CTA), NULL in production
 };
@@ -423,89 +422,6 @@ __device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const floa
     }
 }
 
-// ---- split-K hand-off (epilogue warpgroup, 128 threads): every CTA stores its fp32 partial tile into its own slice of
-//      the tile's workspace (slice = k-slice index); the last CTA to arrive (per-tile counter) adds the slices up in slice
-//      order -- the same order as the cluster exchange, so the result does not depend on which CTA finishes last --, runs
-//      the epilogue and re-zeroes the counter for the next launch.
-//      slice layout (p.ws_tr): float4 group g (= 4 columns) of row r lives at ((g * BM) + r) * 4 floats, so the 32 lanes of
-//      a warp (32 consecutive rows) touch 512 contiguous bytes per store / load -- four full 128-byte lines instead of 32
-//      half-sectors of 32 different lines; ws_tr = 0 keeps the row-major tile (row pitch BN floats).
-__device__ __forceinline__ void stage_ld32(const float* row, int c, uint32_t (&acc)[32]);
-template <int BN, bool kExt>
-__device__ __forceinline__ void splitk_reduce_epilogue(const GemmParams& p, unsigned tile_id, int sp, const float* trow, int r,
-                                                       bool row_valid, long long grow, long long brow, int n0, int ncols_tile,
-                                                       long long d_off, long long r_off, const float* sb, bool r_fast,
-                                                       long long r_row) {
-    const int rs = p.ws_tr ? 4 : BN;             // floats between consecutive rows of one float4 group
-    const int gs = p.ws_tr ? BM * 4 : 4;         // floats between consecutive float4 groups of one row
-    float* slices = p.ws + static_cast<size_t>(tile_id) * p.splits * (BM * BN) + static_cast<size_t>(r) * rs;
-    float* mine = slices + static_cast<size_t>(sp) * (BM * BN);
-#pragma unroll 1
-    for (int c = 0; c * 32 < ncols_tile; ++c) {
-        uint32_t acc[32];
-        stage_ld32(trow, c, acc);
-        if (row_valid) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                __stcg(reinterpret_cast<float4*>(mine + (c * 8 + (j >> 2)) * gs),
-                       make_float4(__uint_as_float(acc[j]), __uint_as_float(acc[j + 1]), __uint_as_float(acc[j + 2]),
-                                   __uint_as_float(acc[j + 3])));
-        }
-    }
-    __threadfence();
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    __shared__ unsigned s_last;
-    if (threadIdx.x == 64) {
-        const unsigned prev = atomicAdd(p.counters + tile_id, 1u);
-        s_last = (prev == static_cast<unsigned>(p.splits) - 1u) ? 1u : 0u;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    const bool last = s_last != 0u;
-    if (!last) return;
-    __threadfence();
-    if (row_valid) {
-        ResidualChunk rc_cur;
-#pragma unroll 1
-        for (int c = 0; c * 32 < ncols_tile; ++c) {
-            const bool pre = r_fast && ncols_tile - c * 32 >= 32;
-            if (pre) residual_prefetch(p, r_row + c * 32, rc_cur);
-            float4 v[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-            for (int s2 = 0; s2 < p.splits; ++s2) {
-                const float* src = slices + static_cast<size_t>(s2) * (BM * BN);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float4 t = __ldcg(reinterpret_cast<const float4*>(src + (c * 8 + j) * gs));
-                    v[j].x += t.x; v[j].y += t.y; v[j].z += t.z; v[j].w += t.w;
-                }
-            }
-            if (p.vec_ok && !p.d_transposed && ncols_tile - c * 32 >= 32) {
-                float f[32];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    f[4 * j] = v[j].x * p.alpha; f[4 * j + 1] = v[j].y * p.alpha;
-                    f[4 * j + 2] = v[j].z * p.alpha; f[4 * j + 3] = v[j].w * p.alpha;
-                }
-                epilogue_chunk32<kExt>(p, f, grow, brow, n0 + c * 32, d_off, r_off, pre ? &rc_cur : nullptr, sb ? sb + c * 32 : nullptr);
-            } else {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const int nc = min(8, ncols_tile - c * 32 - g * 8);
-                    if (nc > 0) {
-                        const float4 lo = v[2 * g], hi = v[2 * g + 1];
-                        float f[8] = {lo.x * p.alpha, lo.y * p.alpha, lo.z * p.alpha, lo.w * p.alpha,
-                                      hi.x * p.alpha, hi.y * p.alpha, hi.z * p.alpha, hi.w * p.alpha};
-                        epilogue_group8<kExt>(p, f, grow, brow, n0 + c * 32 + g * 8, d_off, r_off, nc, nullptr, sb ? sb + c * 32 + g * 8 : nullptr);
-                    }
-                }
-            }
-        }
-    }
-    if (threadIdx.x == 64) p.counters[tile_id] = 0u;   // self-cleaning for the next launch
-}
-
 // Warp roles (384 threads, one CTA per SM):
 //   warpgroup 0 : thread 0 is the TMA producer; after the main loop all 128 threads run the epilogue, one output row each
 //   warpgroups 1, 2 : wgmma consumers, rows [0, 64) and [64, 128) of the tile, fp32 accumulators in registers
@@ -527,6 +443,68 @@ __device__ __forceinline__ void stage_ld32(const float* row, int c, uint32_t (&a
     }
 }
 
+// ---- split-K hand-off through L2 (all 384 threads): every CTA stores its fp32 partial tile into its own slice of the
+//      tile's workspace (slice = k-slice index); the last CTA to arrive (per-tile counter) adds the slices up in slice order,
+//      starting from zero -- the same order as the cluster exchange, so the result does not depend on which CTA finishes
+//      last --, writes the sum back over its staged tile for the ordinary epilogue and re-zeroes the counter.
+//      Slice layout: float4 group g (= 4 columns) of row r is float4 number g * BM + r, so consecutive threads touch
+//      consecutive 16-byte words.  The reduction keeps kU float4 per thread and the next slice's loads in flight while it
+//      adds the current one: the last CTA reads S partial tiles (up to S x 80 KiB) and is bound by L2 latency, not by adds.
+//      Returns false in every CTA but the last one of the tile.
+template <int BN>
+__device__ __forceinline__ bool splitk_reduce_to_stage(const GemmParams& p, unsigned tile_id, int sp, float* stage,
+                                                       int ncols_tile) {
+    constexpr int kPitch = StageCfg<BN>::kPitch;
+    constexpr int kSlice4 = BM * BN / 4;
+    constexpr int kU = 8;
+    const int n4 = ((ncols_tile + 3) >> 2) * BM;        // float4 groups that hold output columns
+    const float4* slices = reinterpret_cast<const float4*>(p.ws) + static_cast<size_t>(tile_id) * p.splits * kSlice4;
+    float4* mine = reinterpret_cast<float4*>(p.ws) + (static_cast<size_t>(tile_id) * p.splits + sp) * kSlice4;
+    for (int i = threadIdx.x; i < n4; i += kThreads)
+        __stcg(mine + i, *reinterpret_cast<const float4*>(stage + (i % BM) * kPitch + 4 * (i / BM)));
+    __threadfence();
+    __syncthreads();
+    __shared__ unsigned s_last;
+    if (threadIdx.x == 0) {
+        const unsigned prev = atomicAdd(p.counters + tile_id, 1u);
+        s_last = (prev == static_cast<unsigned>(p.splits) - 1u) ? 1u : 0u;
+    }
+    __syncthreads();
+    if (s_last == 0u) return false;
+    __threadfence();
+    for (int i0 = threadIdx.x; i0 < n4; i0 += kU * kThreads) {
+        float4 sum[kU], cur[kU], nxt[kU];
+#pragma unroll
+        for (int u = 0; u < kU; ++u) {
+            sum[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+            nxt[u] = sum[u];
+            cur[u] = i0 + u * kThreads < n4 ? __ldcg(slices + i0 + u * kThreads) : sum[u];
+        }
+#pragma unroll 1
+        for (int s = 0; s < p.splits; ++s) {
+            if (s + 1 < p.splits) {
+                const float4* src = slices + static_cast<size_t>(s + 1) * kSlice4;
+#pragma unroll
+                for (int u = 0; u < kU; ++u)
+                    if (i0 + u * kThreads < n4) nxt[u] = __ldcg(src + i0 + u * kThreads);
+            }
+#pragma unroll
+            for (int u = 0; u < kU; ++u) {
+                sum[u].x += cur[u].x; sum[u].y += cur[u].y; sum[u].z += cur[u].z; sum[u].w += cur[u].w;
+                cur[u] = nxt[u];
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kU; ++u) {
+            const int i = i0 + u * kThreads;
+            if (i < n4) *reinterpret_cast<float4*>(stage + (i % BM) * kPitch + 4 * (i / BM)) = sum[u];
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) p.counters[tile_id] = 0u;   // self-cleaning for the next launch
+    return true;
+}
+
 template <int BN, bool A_MN, bool B_MN, int kStages, bool kExt>
 __global__ void __launch_bounds__(kThreads, 1)
 cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -541,7 +519,9 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
 
     const int warp = threadIdx.x >> 5;
-    const int wg = warp >> 2;
+    // warp-uniform as far as the compiler can tell: with a plain threadIdx-derived index the consumer branch counts as
+    // divergent, and ptxas serialises every wgmma.mma_async in it (C7520), waiting for each MMA before issuing the next
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
     if (p.dbg_mode == 3) { pdl_sync(); return; }
     unsigned long long* dbg = p.dbg ? p.dbg + 8ull * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
     if (dbg && threadIdx.x == 0) { dbg[0] = clock64(); dbg[7] = gtimer(); }
@@ -661,6 +641,11 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     named_bar(2, kThreads);        // accumulator tile staged
     if (p.cluster_sk && wg != 0) { cluster_sync_all(); cluster_sync_all(); }   // the two cluster barriers of the epilogue
+    const int ncols_tile = min(BN, p.N - n0);
+    if (p.splits > 1 && !p.cluster_sk && p.dbg_mode == 0) {
+        const unsigned tile_id = (static_cast<unsigned>(bz) * gridDim.y + m_tile) * gridDim.x + blockIdx.x;
+        if (!splitk_reduce_to_stage<BN>(p, tile_id, sp, stage, ncols_tile)) return;
+    }
 
     if (wg == 0) {
         // ===================== epilogue: one output row per thread =====================
@@ -683,7 +668,6 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const long long brow = p.bias_row_div > 0 ? grow / p.bias_row_div : 0;
         const long long d_off = (long long)zo * p.d_bs2 + (long long)zi * p.d_bs;
         const long long r_off = (long long)zo * p.r_bs2 + (long long)zi * p.r_bs;
-        const int ncols_tile = min(BN, p.N - n0);
         // bias row of this tile -> shared memory (global bias loads in the store loop would each wait a full L2 round
         // trip behind the previous chunk's stores)
         __shared__ __align__(16) float s_bias[BN + 8];
@@ -699,11 +683,11 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const bool r_fast = p.R && p.vec_ok && !p.d_transposed && row_valid;
         const long long r_row = r_off + grow * p.ldr + n0;
         ResidualChunk rc_cur, rc_next;
-        if (r_fast && p.splits == 1 && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);
+        if (r_fast && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);
         if (dbg && threadIdx.x == 64) dbg[4] = clock64();
         const float* trow = stage + r * SCfg::kPitch;
         if (p.dbg_mode == 1 || p.dbg_mode == 2) {
-        } else if (p.splits == 1) {
+        } else if (!p.cluster_sk) {     // one k-slice, or the sum of the k-slices (splitk_reduce_to_stage)
 #pragma unroll 1
             for (int c = 0; c * 32 < ncols_tile; ++c) {
                 uint32_t acc[32];
@@ -744,7 +728,7 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
                 rc_cur = rc_next;
             }
-        } else if (p.cluster_sk) {
+        } else {
             // ---- split-K inside a thread-block cluster: the `splits` CTAs of this tile are the cluster (1,1,splits), rank =
             //      k-slice.  The 8-column groups of the tile are dealt round-robin to the CTAs (group g -> CTA g % S); every CTA
             //      sends each group of its partial accumulator into the owner's exchange buffer (the part of the idle TMA ring
@@ -787,10 +771,6 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                                           sb ? sb + g * 8 : nullptr);
                 }
             }
-        } else {
-            const unsigned tile_id = (static_cast<unsigned>(bz) * gridDim.y + m_tile) * gridDim.x + blockIdx.x;
-            splitk_reduce_epilogue<BN, kExt>(p, tile_id, sp, trow, r, row_valid, grow, brow, n0, ncols_tile, d_off, r_off, sb,
-                                             r_fast, r_row);
         }
         if (dbg && threadIdx.x == 64) dbg[5] = clock64();
     }
@@ -1137,10 +1117,6 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
 
     // ---- split-K heuristic: fill the SMs when the tile grid alone cannot (bs=1 low-resolution layers) ----
     p.force_stages = (d.stages == 3 || d.stages == 6) ? d.stages : 0;
-    {
-        static const int ws_tr = getenv("CB_GEMM_WS_TR") ? atoi(getenv("CB_GEMM_WS_TR")) : 1;   // A/B aid
-        p.ws_tr = ws_tr;
-    }
     p.splits = 1;
     p.kiters_per_split = p.taps * p.kchunks;
     {

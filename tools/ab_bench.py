@@ -1,4 +1,4 @@
-"""A/B bench.py environment knobs on one box: python tools/ab_bench.py - CB_FE_CTAS=48 CB_GEMM_WS_TR=0,CB_FE_CTAS=64 [-- extra
+"""A/B bench.py environment knobs on one box: python tools/ab_bench.py - CB_FE_CTAS=48 CB_GEMM_CLUSTER_SK=0,CB_FE_CTAS=64 [-- extra
 bench args].  Every argument is one configuration (comma-separated KEY=VALUE pairs, "-" = the defaults); one JSON line each."""
 import json, os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
