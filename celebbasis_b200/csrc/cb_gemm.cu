@@ -505,6 +505,34 @@ __device__ __forceinline__ bool splitk_reduce_to_stage(const GemmParams& p, unsi
     return true;
 }
 
+// One k-iteration of a consumer warpgroup: KSTEPS k16 MMAs over the stage at (a_src, b_src), issued as one wgmma group.
+// Straight-line code between one fence and one commit lets ptxas put a single warpgroup.arrive in front of the batch and
+// the scoreboard wait (gsb0) on its last MMA only; an MMA in a branch of its own gets an injected arrive (C7519) and waits
+// for the one before it.
+template <int BN, bool A_MN, bool B_MN, bool BF16, int KSTEPS>
+__device__ __forceinline__ void mma_batch(float (&acc)[BN / 2], uint32_t a_src, uint32_t b_src) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) {
+        const uint64_t adesc = A_MN ? gmma_desc_sw128(a_src + k * 2048, 8192, 1024) : gmma_desc_sw128(a_src + k * 32, 16, 1024);
+        const uint64_t bdesc = B_MN ? gmma_desc_sw128(b_src + k * 2048, 8192, 1024) : gmma_desc_sw128(b_src + k * 32, 16, 1024);
+        Wgmma<BN, BF16, A_MN, B_MN>::mma(acc, adesc, bdesc, 1u);
+    }
+    wgmma_commit();
+}
+
+// ksteps < 4 only in the last 64-chunk of a tap (K % 64 != 0); it gets exactly that many MMAs, never zero-filled extra
+// ones: a +0 product would turn a -0.0 accumulator into +0.0
+template <int BN, bool A_MN, bool B_MN, bool BF16>
+__device__ __forceinline__ void mma_kiter(float (&acc)[BN / 2], uint32_t a_src, uint32_t b_src, int ksteps) {
+    switch (ksteps) {
+        case 4: mma_batch<BN, A_MN, B_MN, BF16, 4>(acc, a_src, b_src); break;
+        case 3: mma_batch<BN, A_MN, B_MN, BF16, 3>(acc, a_src, b_src); break;
+        case 2: mma_batch<BN, A_MN, B_MN, BF16, 2>(acc, a_src, b_src); break;
+        default: mma_batch<BN, A_MN, B_MN, BF16, 1>(acc, a_src, b_src); break;
+    }
+}
+
 template <int BN, bool A_MN, bool B_MN, int kStages, bool kExt>
 __global__ void __launch_bounds__(kThreads, 1)
 cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -550,7 +578,7 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 256);     // every consumer thread releases the stage
+            mbar_init(empty_bar(s), 8);       // lane 0 of each of the 8 consumer warps releases the stage
         }
         mbar_fence_init();
         fence_proxy_async_smem();
@@ -566,19 +594,21 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (wg == 0) {
         if (threadIdx.x == 0) {
             // ===================== TMA producer =====================
+            // ring slot, its phase bit and the (tap row r, tap column sx, 64-chunk kc) of the k-iteration are counters
+            // stepped once per iteration: no integer division in the loop
+            int s = 0;
+            uint32_t ph = 0;
+            int tap = it0 / p.kchunks;
+            int kc = it0 - tap * p.kchunks;
+            int r = tap / p.kw;
+            int sx = tap - r * p.kw;
             for (int it = it0; it < it1; ++it) {
-                const int li = it - it0;
-                const int s = li % kStages;
-                const uint32_t ph = (li / kStages) & 1;
                 mbar_wait(empty_bar(s), ph ^ 1u);
                 mbar_arrive_expect_tx(full_bar(s), p.a_bytes + p.b_bytes);
-                const int tap = it / p.kchunks;
-                const int kc = it - tap * p.kchunks;
                 const uint32_t a_dst = smem_base + s * Cfg::kStageBytes;
                 const uint32_t b_dst = a_dst + Cfg::kABytes;
                 const int tap_b = p.flip_taps ? (p.taps - 1 - tap) : tap;
                 if (p.conv) {
-                    const int r = tap / p.kw, sx = tap - r * p.kw;
                     tma_load_4d(a_dst, &tmA, full_bar(s), kc * BK, ow0 * p.stride + sx - p.pad_left,
                                 oh0 * p.stride + r - p.pad_top, img0);
                 } else if (A_MN) {
@@ -595,6 +625,12 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 } else {
                     tma_load_4d(b_dst, &tmB, full_bar(s), kc * BK, tap_b * p.b_tap_rows + n0, zi, zo);
                 }
+                if (++s == kStages) { s = 0; ph ^= 1u; }
+                if (++kc == p.kchunks) {
+                    kc = 0;
+                    ++tap;
+                    if (++sx == p.kw) { sx = 0; ++r; }
+                }
             }
         }
         __syncwarp();
@@ -604,31 +640,31 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         const uint32_t a_half = static_cast<uint32_t>(wg - 1) * 8192u;     // this warpgroup's 64 rows of the A tile
+        // wgmma.wait_group is warp-collective, so once it returns one lane's arrival releases the stage for its warp
+        const bool releaser = (threadIdx.x & 31) == 0;
+        int s = 0, s_prev = 0;
+        uint32_t ph = 0;
+        int kc = it0 % p.kchunks;
         for (int it = it0; it < it1; ++it) {
-            const int li = it - it0;
-            const int s = li % kStages;
-            mbar_wait(full_bar(s), (li / kStages) & 1);
-            if (dbg && li == 0 && threadIdx.x == 128) dbg[2] = clock64();
+            mbar_wait(full_bar(s), ph);
+            if (dbg && it == it0 && threadIdx.x == 128) dbg[2] = clock64();
             const uint32_t a_src = smem_base + s * Cfg::kStageBytes + a_half;
             const uint32_t b_src = smem_base + s * Cfg::kStageBytes + Cfg::kABytes;
-            const int kc = it % p.kchunks;
             const int ksteps = (kc == p.kchunks - 1) ? p.ksteps_last : (BK / 16);
             wgmma_fence_regs(acc);
-            wgmma_fence();
-            for (int k = 0; k < ksteps; ++k) {
-                const uint64_t adesc = A_MN ? gmma_desc_sw128(a_src + k * 2048, 8192, 1024) : gmma_desc_sw128(a_src + k * 32, 16, 1024);
-                const uint64_t bdesc = B_MN ? gmma_desc_sw128(b_src + k * 2048, 8192, 1024) : gmma_desc_sw128(b_src + k * 32, 16, 1024);
-                wgmma_any<BN, A_MN, B_MN>(p.bf16 != 0, acc, adesc, bdesc, 1u);
-            }
-            wgmma_commit();
+            if (p.bf16) mma_kiter<BN, A_MN, B_MN, true>(acc, a_src, b_src, ksteps);
+            else mma_kiter<BN, A_MN, B_MN, false>(acc, a_src, b_src, ksteps);
             // keep one k-iteration of MMAs in flight: the previous stage is released once its group has retired
             wgmma_wait<1>();
             wgmma_fence_regs(acc);
-            if (li > 0) mbar_arrive(empty_bar((li - 1) % kStages));
+            if (it > it0 && releaser) mbar_arrive(empty_bar(s_prev));
+            s_prev = s;
+            if (++s == kStages) { s = 0; ph ^= 1u; }
+            if (++kc == p.kchunks) kc = 0;
         }
         wgmma_wait<0>();
         wgmma_fence_regs(acc);
-        if (it1 > it0) mbar_arrive(empty_bar((it1 - it0 - 1) % kStages));
+        if (it1 > it0 && releaser) mbar_arrive(empty_bar(s_prev));
         if (dbg && threadIdx.x == 128) dbg[3] = clock64();
         named_bar(4, 256);          // both warpgroups' MMAs have read the ring for the last time
         const int l = threadIdx.x & 31, w = warp & 3;
