@@ -5,40 +5,48 @@
 // (heads x N x N) score tensor -- 512 MiB fp32 per 4096-token block in the reference -- never reaches HBM unless
 // the caller asks for the probabilities (training keeps them for the backward pass).
 //
-// One CTA = 128 query rows of one (image, head):
-//   warp 8        : TMA producer -- Q once, then K_j / V_j blocks of 64 keys through a 3-stage mbarrier ring
-//   warpgroups 0,1: query rows [0, 64) / [64, 128).  Per block: S_j = Q K_j^T with wgmma (fp32 in registers), online
+// One CTA = 128 query rows of one (image, head), three warpgroups:
+//   warpgroup 0   : TMA producer (one elected thread) -- Q once, then K_j / V_j blocks of 64 keys through a 4-stage
+//                   mbarrier ring.  It hands most of its registers to the consumers (setmaxnreg).
+//   warpgroups 1,2: query rows [0, 64) / [64, 128).  Per block: S_j = Q K_j^T with wgmma (fp32 in registers), online
 //                   softmax on the register fragment (running max / sum per row, exp2 with the scale folded in, row
 //                   reductions across the four lanes that share a row), P_j written as a K-major SWIZZLE_128B A tile in
 //                   shared memory, O += P_j V_j with wgmma (V read MN-major straight from its [keys][d] layout, O in
 //                   registers); finally O / l -> HBM and logsumexp.
+//                   Pipelined within the warpgroup: O += P_{j-1} V_{j-1} is queued behind S_j and stays in flight while
+//                   the softmax of block j runs, so the tensor cores and the exp unit work at the same time.
 // Head dims 40 / 64 / 80 / 128 (any multiple of 8 up to 128): the tensor maps declare the head's d columns as the
-// K extent, so TMA zero-fills the rest of each 64-column box and the MMAs run on 16-column multiples.
+// K extent, so TMA zero-fills the rest of each 64-column box and the MMAs run on 16-column multiples.  The number of
+// those k16 steps is a template parameter, so every MMA group is one straight-line batch.
 #include <string.h>
+
+#include <type_traits>
 
 #include "cb_common.cuh"
 
 namespace cb {
 
 constexpr int kAttnConsumers = 256;                  // two wgmma warpgroups
-constexpr int kAttnThreads = kAttnConsumers + 32;    // + the TMA producer warp
+constexpr int kAttnThreads = kAttnConsumers + 128;   // + the TMA producer warpgroup
+// Register split of the 384-thread CTA (65,536 registers): ptxas budgets 168 per thread for three warpgroups; the
+// producer drops to 24 and the two consumer warpgroups rise to 240 (128 * 24 + 256 * 240 = 64,512).
+constexpr int kAttnProducerRegs = 24;
+constexpr int kAttnConsumerRegs = 240;
 constexpr int kBQ = 128;    // query rows per CTA
 constexpr int kBKV = 64;    // keys per block
 
 struct AttnParams {
     int nq, nk, heads, images;
-    int d, dpad16;          // head dim, head dim rounded up to 16
-    int dboxes;             // 64-column boxes per row of Q/K/V (1 or 2)
+    int d;                  // head dim
     int causal;
     int two_pass;           // pass A: row max / sum only; pass B: normalised probabilities (needed when P is stored)
     float scale_log2e;      // scale * log2(e)
     void* O;
-    int o_dtype;
     long long ldo;          // elements between consecutive query rows of O
     float* lse;             // [images][heads][nq] natural-log sum-exp (scaled scores), or NULL
     void* P;                // optional probabilities [images*heads][nq][ldp] (same 16-bit dtype as the operands)
     long long ldp;
-    int p_is_bf16;
+    int is_bf16;            // operands, O and P are bf16 (else fp16)
 };
 
 template <int DBOX>  // number of 64-column boxes of the head dim (1: d <= 64, 2: d <= 128)
@@ -47,9 +55,60 @@ struct AttnCfg {
     static constexpr int kKBytes = DBOX * kBKV * 128;
     static constexpr int kVBytes = DBOX * kBKV * 128;
     static constexpr int kPBytes = kBQ * 128;              // 64 keys = one 128-byte chunk per query row
-    static constexpr int kStages = 3;
+    // K_j / V_j stay resident until O += P_j V_j retires during block j+1; the other stages are the producer's lead
+    static constexpr int kStages = 4;
     static constexpr int kSmemBytes = kQBytes + kStages * (kKBytes + kVBytes) + 2 * kPBytes + 1024 + 256;   // two P buffers
 };
+
+// Consumer-side mbarrier wait.  Unlike mbar_wait it has no __trap() hang guard: a trap reachable from the consumer
+// region makes ptxas ignore the setmaxnreg.inc budget and allocate the consumers within the 168 registers of a
+// 384-thread CTA, which spills the backward's dK/dV accumulators and serialises their wgmmas (C7512).
+__device__ __forceinline__ void mbar_wait_consumer(uint32_t bar, uint32_t parity) {
+    while (!mbar_try_wait(bar, parity)) {
+    }
+}
+
+template <uint32_t R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// acc[64 x 64] (+)= A B^T over KS k16 steps, one wgmma group: A = 64 rows at a, B = 64 rows at b, both K-major
+// SWIZZLE_128B with the head dim split into 64-column boxes a_box / b_box bytes apart.  k = 0 overwrites acc.
+// Straight-line code between one fence and one commit gets one warpgroup.arrive for the whole batch; an MMA in a
+// branch of its own gets an injected arrive (C7519) and waits for the one before it.
+template <int KS, bool BF16>
+__device__ __forceinline__ void mma_rows(float (&acc)[32], uint32_t a, uint32_t a_box, uint32_t b, uint32_t b_box) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KS; ++k)
+        Wgmma<64, BF16, 0, 0>::mma(acc, gmma_desc_sw128(a + (k >> 2) * a_box + (k & 3) * 32, 16, 1024),
+                                   gmma_desc_sw128(b + (k >> 2) * b_box + (k & 3) * 32, 16, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+}
+template <int KS>
+__device__ __forceinline__ void mma_rows_any(bool bf16, float (&acc)[32], uint32_t a, uint32_t a_box, uint32_t b,
+                                             uint32_t b_box) {
+    if (bf16) mma_rows<KS, true>(acc, a, a_box, b, b_box);
+    else mma_rows<KS, false>(acc, a, a_box, b, b_box);
+}
+// acc[64 x NO] (+)= A Y over one 64-item block, one wgmma group: A = [64 rows][64 items] K-major at a (16-item step k),
+// Y = [64 items][NO] MN-major at y (16 items = 2 groups of 8 rows, SBO 1024; 64-column chunks at LBO).
+// acc_in = 0 overwrites acc with the first product.
+template <int NO, bool BF16>
+__device__ __forceinline__ void mma_block(float (&acc)[NO / 2], uint32_t a, uint32_t y, uint32_t acc_in) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBKV / 16; ++k)
+        Wgmma<NO, BF16, 0, 1>::mma(acc, gmma_desc_sw128(a + k * 32, 16, 1024), gmma_desc_sw128(y + k * 2048, kBKV * 128, 1024),
+                                   k > 0 ? 1u : acc_in);
+    wgmma_commit();
+}
+template <int NO>
+__device__ __forceinline__ void mma_block_any(bool bf16, float (&acc)[NO / 2], uint32_t a, uint32_t y, uint32_t acc_in) {
+    if (bf16) mma_block<NO, true>(acc, a, y, acc_in);
+    else mma_block<NO, false>(acc, a, y, acc_in);
+}
 
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
@@ -78,10 +137,11 @@ __device__ __forceinline__ float quad_sum(float v) {
     return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <int DBOX>
+template <int KS>   // k16 steps of the head dim: ceil(d / 16)
 __global__ void __launch_bounds__(kAttnThreads, 1)
 cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p) {
+    constexpr int DBOX = (KS + 3) / 4;
     using Cfg = AttnCfg<DBOX>;
     constexpr int kSt = Cfg::kStages;
     constexpr int NO = DBOX * 64;                 // output columns (zero-filled past d)
@@ -96,6 +156,8 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     auto bar_kv_empty = [&](int s) { return bars + 8u * (1 + kSt + s); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // warp-uniform as far as the compiler can tell (a plain threadIdx-derived index makes the role branch divergent)
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
     const int q0 = blockIdx.x * kBQ;
     const int head = blockIdx.y, img = blockIdx.z;
     int nblk = (p.nk + kBKV - 1) / kBKV;
@@ -118,8 +180,9 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     __syncthreads();
     pdl_sync();
 
-    if (warp == kAttnConsumers / 32) {
-        if (lane == 0) {
+    if (wg == 0) {
+        regs_dealloc<kAttnProducerRegs>();
+        if (threadIdx.x == 0) {
             // ============================ TMA producer ============================
             mbar_arrive_expect_tx(bar_q, Cfg::kQBytes);
 #pragma unroll
@@ -141,35 +204,44 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
         }
         return;
     }
+    regs_alloc<kAttnConsumerRegs>();
 
     // ============================ consumers: 64 query rows per warpgroup ============================
-    const int wg = warp >> 2;
-    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
+    const int cw = wg - 1;
+    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
     const int cq = 2 * (lane & 3);                             // this thread's first column in every 8-column group
-    const bool bf16 = p.p_is_bf16 != 0;
-    const uint32_t qoff = static_cast<uint32_t>(wg) * 8192u;   // this warpgroup's 64 rows of a 128-row tile
+    const bool bf16 = p.is_bf16 != 0;
+    const uint32_t qoff = static_cast<uint32_t>(cw) * 8192u;   // this warpgroup's 64 rows of a 128-row tile
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, inv_l[2] = {1.f, 1.f};
     float o[NO / 2];
 #pragma unroll
     for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
-    const int ks_qk = p.dpad16 / 16;
-    mbar_wait(bar_q, 0);
-    for (int vj = 0; vj < nv; ++vj) {
+
+    // Per block vj: S_vj = Q K_vj^T is issued, then O += P_{vj-1} V_{vj-1} behind it; the softmax of block vj runs once
+    // S_vj has retired, while the PV group is still on the tensor cores.  That group retires before O is rescaled and
+    // P_vj is handed to the next block; only then is the K/V stage of block vj-1 released.
+    // Whether a PV group is pending is known at compile time in each of the three loops below: a wgmma wait under a
+    // runtime condition counts as divergent, and ptxas then serialises the MMAs (C7518).
+    int pv_stage = 0, pv_j = 0;                    // P_{vj-1} in shared memory, waiting for its PV group
+    auto issue_pv = [&]() {
+        wgmma_fence_regs(o);
+        mma_block_any<NO>(bf16, o, sP + (pv_j & 1) * Cfg::kPBytes + qoff,
+                          sKV + pv_stage * (Cfg::kKBytes + Cfg::kVBytes) + Cfg::kKBytes, 1u);
+    };
+    float sc[32];
+    auto block = [&](int vj, auto pv_pending_c) {
+        constexpr bool pv_pending = decltype(pv_pending_c)::value;
         const bool full = vj >= nstat;
         const int j = full ? vj - nstat : vj;
         const int s = vj % kSt;
-        mbar_wait(bar_kv_full(s), (vj / kSt) & 1);
-        const uint32_t aK = sKV + s * (Cfg::kKBytes + Cfg::kVBytes), aV = aK + Cfg::kKBytes;
-        float sc[32];
-        wgmma_fence();
-        for (int k = 0; k < ks_qk; ++k) {
-            const uint32_t offq = (k >> 2) * (kBQ * 128) + qoff + (k & 3) * 32;    // 64-col box, then 16-col step
-            const uint32_t offk = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-            wgmma_any<64, 0, 0>(bf16, sc, gmma_desc_sw128(sQ + offq, 16, 1024), gmma_desc_sw128(aK + offk, 16, 1024),
-                                k > 0 ? 1u : 0u);
+        mbar_wait_consumer(bar_kv_full(s), (vj / kSt) & 1);
+        mma_rows_any<KS>(bf16, sc, sQ + qoff, kBQ * 128, sKV + s * (Cfg::kKBytes + Cfg::kVBytes), kBKV * 128);
+        if constexpr (pv_pending) {
+            issue_pv();
+            wgmma_wait<1>();                       // S_vj has retired; O += P_{vj-1} V_{vj-1} may still run
+        } else {
+            wgmma_wait<0>();
         }
-        wgmma_commit();
-        wgmma_wait<0>();
         wgmma_fence_regs(sc);
         if (!full) mbar_arrive(bar_kv_empty(s));          // statistics pass: the K stage is free once S is done
         const int kbase = j * kBKV;
@@ -191,25 +263,20 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
             mx[h] = quad_max(mh) * p.scale_log2e;
         }
         const bool online = !(p.two_pass && full);      // running max / sum still being built
-        float m_use[2];
+        float m_use[2], corr[2] = {1.f, 1.f};
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             if (online) {
                 // Lazy rescale: the reference maximum only moves when the block maximum exceeds it by more than 2^8
                 // (probabilities stay <= 256, exact in fp16/fp32).
                 const float m_new = fmaxf(m[h], mx[h]);
-                float corr = 1.f;
                 if (m[h] == -INFINITY) {
                     m[h] = m_new;                            // first block: nothing accumulated yet (l = 0, O zero)
                 } else if (m_new > m[h] + 8.f) {
-                    corr = fast_exp2(m[h] - m_new);
+                    corr[h] = fast_exp2(m[h] - m_new);
                     m[h] = m_new;
                 }
-                l[h] *= corr;
-                if (full && corr != 1.f) {
-#pragma unroll
-                    for (int jj = 0; jj < NO / 8; ++jj) { o[4 * jj + 2 * h] *= corr; o[4 * jj + 2 * h + 1] *= corr; }
-                }
+                l[h] *= corr[h];
             }
             m_use[h] = (m[h] == -INFINITY) ? 0.f : m[h];  // (fully masked so far: the exponent argument stays -inf)
         }
@@ -227,9 +294,10 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
                     inv_l[h] = l[h] > 0.f ? 1.f / l[h] : 0.f;
                 }
             }
-            continue;
+            return;
         }
-        // P = exp2(s - m) (normalised by 1/l in two-pass mode): swizzled K-major A tile in smem (+ optional HBM copy)
+        // P = exp2(s - m) (normalised by 1/l in two-pass mode): swizzled K-major A tile in smem (+ optional HBM copy).
+        // Buffer j & 1 was last read by O += P_{j-2} V_{j-2}, which retired in the previous block.
         const uint32_t tile = sP + (j & 1) * Cfg::kPBytes;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -251,22 +319,30 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
             }
             if (online) l[h] += rs;
         }
-        fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        named_bar(1 + wg, 128);         // this warpgroup's 64 rows of P are complete
-        wgmma_fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kBKV / 16; ++k) {
-            // A = P [64 rows][64 keys] K-major: 16-key step k;  B = V [64 keys][d] MN-major: 16 keys = 2 groups of 8 rows
-            // (SBO 1024), 64-col chunks at LBO
-            wgmma_any<NO, 0, 1>(bf16, o, gmma_desc_sw128(tile + qoff + k * 32, 16, 1024),
-                                gmma_desc_sw128(aV + k * 2048, kBKV * 128, 1024), 1u);
+        if constexpr (pv_pending) {
+            wgmma_wait<0>();                       // O += P_{vj-1} V_{vj-1} has retired
+            wgmma_fence_regs(o);
+            mbar_arrive(bar_kv_empty(pv_stage));   // K_{vj-1} / V_{vj-1} stage reusable
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(o);
-        mbar_arrive(bar_kv_empty(s));   // K_j / V_j stage reusable
-    }
+        if (online) {                              // x * 1.0f is exact: rows whose maximum did not move keep their bits
+#pragma unroll
+            for (int jj = 0; jj < NO / 8; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) { o[4 * jj + 2 * h] *= corr[h]; o[4 * jj + 2 * h + 1] *= corr[h]; }
+        }
+        fence_proxy_async_smem();       // generic-proxy smem writes -> visible to the tensor core (async proxy)
+        named_bar(1 + cw, 128);         // this warpgroup's 64 rows of P are complete
+        pv_stage = s;
+        pv_j = j;
+    };
+    mbar_wait_consumer(bar_q, 0);
+    int vj = 0;
+    for (; vj < nstat; ++vj) block(vj, std::false_type{});     // statistics pass (two-pass mode)
+    block(vj++, std::false_type{});                            // first full block: nothing to accumulate yet
+    for (; vj < nv; ++vj) block(vj, std::true_type{});
+    issue_pv();                                                // there is always at least one full block
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
     // ---- epilogue: O / l, logsumexp ----
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -282,7 +358,7 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
         for (int jj = 0; jj < NO / 8; ++jj) {
             const int col = jj * 8 + cq;
             if (col < p.d)
-                *reinterpret_cast<uint32_t*>(orow + col) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, p.o_dtype == CB_BF16);
+                *reinterpret_cast<uint32_t*>(orow + col) = pack2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv, bf16);
         }
     }
 }
@@ -290,12 +366,12 @@ cb_attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 int make_tmap(CUtensorMap* out, int dtype, int rank, const void* ptr, const uint64_t* dims,
               const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* estr);
 
-template <int DBOX>
+template <int KS>
 static int launch_attn(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, const AttnParams& p, dim3 grid,
                        cudaStream_t st) {
-    using Cfg = AttnCfg<DBOX>;
+    using Cfg = AttnCfg<(KS + 3) / 4>;
     static bool done = false;
-    auto kern = cb_attention_fwd_kernel<DBOX>;
+    auto kern = cb_attention_fwd_kernel<KS>;
     if (!done) {
         CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
         done = true;
@@ -317,9 +393,11 @@ static int launch_attn(const CUtensorMap& q, const CUtensorMap& k, const CUtenso
 // K-major SWIZZLE_128B A tiles; then  MODE 0: acc += dS Y1 (= dS K);  MODE 1: accV += P^T Y2 (= P^T dO),
 // accK += dS^T Y1 (= dS^T Q) with the streamed tiles read MN-major, exactly like V in the forward kernel.
 // MODE 0 also computes delta (it owns dO and reads O) and stores it for the MODE 1 launch that follows it in stream order.
+// The CTA layout and register split are the forward kernel's.  T1 and T2 are issued back to back, so P is computed
+// while T2 runs; the accumulation group of block j stays in flight until block j+1's T1 has retired.
 struct AttnBwdParams {
     int n_stat, n_stream, heads, images;     // rows of the stationary / streamed operands (nq,nk in MODE 0; nk,nq in MODE 1)
-    int d, dpad16, dboxes, causal;
+    int d, causal;
     float scale, scale_log2e;
     const float* lse;        // [images][heads][nq]
     float* delta;            // [images][heads][nq]   (written by MODE 0, read by MODE 1)
@@ -345,11 +423,27 @@ struct AttnBwdCfg {
     static constexpr int kSmemBytes = 2 * kXBytes + 2 * 2 * kYBytes + kNumA * kABytes + 1024 + 256;
 };
 
-template <int DBOX, int MODE>
+// MODE 1's two accumulations of one block as one wgmma group (k-order within each accumulator as in mma_block)
+template <int NO, bool BF16>
+__device__ __forceinline__ void mma_block2(float (&acc0)[NO / 2], uint32_t a0, uint32_t y0, float (&acc1)[NO / 2],
+                                           uint32_t a1, uint32_t y1, uint32_t acc_in) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBKV / 16; ++k) {
+        Wgmma<NO, BF16, 0, 1>::mma(acc0, gmma_desc_sw128(a0 + k * 32, 16, 1024), gmma_desc_sw128(y0 + k * 2048, kBKV * 128, 1024),
+                                   k > 0 ? 1u : acc_in);
+        Wgmma<NO, BF16, 0, 1>::mma(acc1, gmma_desc_sw128(a1 + k * 32, 16, 1024), gmma_desc_sw128(y1 + k * 2048, kBKV * 128, 1024),
+                                   k > 0 ? 1u : acc_in);
+    }
+    wgmma_commit();
+}
+
+template <int KS, int MODE>   // KS: k16 steps of the head dim, ceil(d / 16)
 __global__ void __launch_bounds__(kAttnThreads, 1)
 cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                         const __grid_constant__ CUtensorMap tmY1, const __grid_constant__ CUtensorMap tmY2,
                         const __grid_constant__ AttnBwdParams p) {
+    constexpr int DBOX = (KS + 3) / 4;
     using Cfg = AttnBwdCfg<DBOX, MODE>;
     constexpr int NO = DBOX * 64;
     extern __shared__ uint8_t smem_raw[];
@@ -364,6 +458,7 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
     __shared__ float2 s_stat[2][kBKV];         // MODE 1: (lse*log2e, delta*scale) of the streamed queries, per warpgroup
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
     const int x0 = blockIdx.x * kBQ;
     const int head = blockIdx.y, img = blockIdx.z;
     // streamed block range (causal: keys <= query)
@@ -384,8 +479,9 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
     __syncthreads();
     pdl_sync();
 
-    if (warp == kAttnConsumers / 32) {
-        if (lane == 0) {
+    if (wg == 0) {
+        regs_dealloc<kAttnProducerRegs>();
+        if (threadIdx.x == 0) {
             mbar_arrive_expect_tx(bar_x, 2 * Cfg::kXBytes);
 #pragma unroll
             for (int b = 0; b < DBOX; ++b) {
@@ -406,14 +502,15 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
         }
         return;
     }
+    regs_alloc<kAttnConsumerRegs>();
 
     // ====================== consumers: 64 stationary rows per warpgroup ======================
-    const int wg = warp >> 2;
-    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
+    const int cw = wg - 1;
+    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of fragment half 0 (half 1: rl + 8)
     const int cq = 2 * (lane & 3);
     const int et = threadIdx.x & 127;                          // thread index inside the warpgroup
     const bool bf16 = p.is_bf16 != 0;
-    const uint32_t xoff = static_cast<uint32_t>(wg) * 8192u;
+    const uint32_t xoff = static_cast<uint32_t>(cw) * 8192u;
     const long long stat_base = (static_cast<long long>(img) * p.heads + head) * p.nq;
     const float kLog2e = 1.4426950408889634f;
     float lse_r[2] = {0.f, 0.f}, delta_r[2] = {0.f, 0.f};     // MODE 0: this thread's query rows' statistics
@@ -449,24 +546,26 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
         }
     }
     // acc1: MODE 1 only.  Neither is initialised: the first block's MMAs overwrite them (scale_d = 0), and an accumulator
-    // written by ordinary instructions would make ptxas serialise every wgmma of the loop.
+    // written by ordinary instructions would make ptxas serialise every wgmma of the loop.  For the same reason P lives in
+    // registers of its own, not in T1's accumulator.
     float acc0[NO / 2], acc1[NO / 2];
-    const int ks = p.dpad16 / 16;
-    mbar_wait(bar_x, 0);
+    mbar_wait_consumer(bar_x, 0);
     for (int it = 0; it < nit; ++it) {
         const int j = jbeg + it;
         const int cbase = j * kBKV;
         const int s = it & 1;
         if (MODE == 1 && et < kBKV) {
             const int qc = cbase + et;
-            s_stat[wg][et] = qc < p.n_stream ? make_float2(p.lse[stat_base + qc] * kLog2e, p.delta[stat_base + qc] * p.scale)
+            s_stat[cw][et] = qc < p.n_stream ? make_float2(p.lse[stat_base + qc] * kLog2e, p.delta[stat_base + qc] * p.scale)
                                              : make_float2(0.f, 0.f);
         }
-        // the statistics are in place, and every thread of this warpgroup is past the previous block's accumulation MMAs
-        // (the A tiles below may be overwritten)
-        named_bar(1 + wg, 128);
-        mbar_wait(bar_y_full(s), (it >> 1) & 1);
+        named_bar(1 + cw, 128);                    // the statistics are in place
+        mbar_wait_consumer(bar_y_full(s), (it >> 1) & 1);
         const uint32_t y1 = sY + s * 2 * Cfg::kYBytes, y2 = y1 + Cfg::kYBytes;
+        // groups in flight: [accumulation of block j-1], T1, T2
+        float t[32], t2[32];
+        mma_rows_any<KS>(bf16, t, sX1 + xoff, kBQ * 128, y1, kBKV * 128);
+        mma_rows_any<KS>(bf16, t2, sX2 + xoff, kBQ * 128, y2, kBKV * 128);
         // valid streamed items of this block for each of this thread's rows
         int cvalid[2], cfirst[2];
 #pragma unroll
@@ -480,17 +579,11 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
             }
             if (MODE == 0 && xrow >= p.n_stat) cvalid[h] = 0;
         }
-        float t[32];
-        wgmma_fence();
-        for (int k = 0; k < ks; ++k) {
-            const uint32_t offx = (k >> 2) * (kBQ * 128) + xoff + (k & 3) * 32;
-            const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-            wgmma_any<64, 0, 0>(bf16, t, gmma_desc_sw128(sX1 + offx, 16, 1024), gmma_desc_sw128(y1 + offy, 16, 1024), k > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
+        wgmma_wait<1>();                           // T1 and the accumulation of block j-1 have retired
         wgmma_fence_regs(t);
-        // P = ex2(fma(T1, scale*log2e, -lse*log2e)), zero outside the valid block items
+        if (it > 0) mbar_arrive(bar_y_empty(s ^ 1));   // Y_{j-1} stage reusable
+        // P = ex2(fma(T1, scale*log2e, -lse*log2e)), zero outside the valid block items, computed while T2 runs
+        float pr[32];
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
@@ -498,24 +591,19 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
                     const int col = jj * 8 + cq + c;
-                    const float l2 = MODE == 0 ? lse_r[h] : s_stat[wg][col].x;
+                    const float l2 = MODE == 0 ? lse_r[h] : s_stat[cw][col].x;
                     const float pv = fast_exp2(fmaf(t[4 * jj + 2 * h + c], p.scale_log2e, -l2));
-                    t[4 * jj + 2 * h + c] = (col < cvalid[h] && col >= cfirst[h]) ? pv : 0.f;
+                    pr[4 * jj + 2 * h + c] = (col < cvalid[h] && col >= cfirst[h]) ? pv : 0.f;
                 }
+        // The A tiles were last read by the accumulation group of block j-1, which wgmma_wait<1> above retired.  A
+        // wgmma group completes as one warpgroup-wide operation, so once this warp has seen it retire, none of the
+        // group's reads of all 64 rows is still pending, and no warpgroup barrier is needed before the tiles are rewritten.
         if (MODE == 1) {
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) st_a_pair(sA, rl + 8 * h, jj * 8 + cq, pack2(t[4 * jj + 2 * h], t[4 * jj + 2 * h + 1], bf16));
+                for (int h = 0; h < 2; ++h) st_a_pair(sA, rl + 8 * h, jj * 8 + cq, pack2(pr[4 * jj + 2 * h], pr[4 * jj + 2 * h + 1], bf16));
         }
-        float t2[32];
-        wgmma_fence();
-        for (int k = 0; k < ks; ++k) {
-            const uint32_t offx = (k >> 2) * (kBQ * 128) + xoff + (k & 3) * 32;
-            const uint32_t offy = (k >> 2) * (kBKV * 128) + (k & 3) * 32;
-            wgmma_any<64, 0, 0>(bf16, t2, gmma_desc_sw128(sX2 + offx, 16, 1024), gmma_desc_sw128(y2 + offy, 16, 1024), k > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(t2);
         // dS = P * fma(T2, scale, -delta*scale)
@@ -531,8 +619,8 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
                 float ds[2];
 #pragma unroll
                 for (int c = 0; c < 2; ++c) {
-                    const float dl = MODE == 0 ? delta_r[h] : s_stat[wg][jj * 8 + cq + c].y;
-                    ds[c] = t[4 * jj + 2 * h + c] * fmaf(t2[4 * jj + 2 * h + c], p.scale, -dl);
+                    const float dl = MODE == 0 ? delta_r[h] : s_stat[cw][jj * 8 + cq + c].y;
+                    ds[c] = pr[4 * jj + 2 * h + c] * fmaf(t2[4 * jj + 2 * h + c], p.scale, -dl);
                 }
                 const uint32_t v = pack2(ds[0], ds[1], bf16);
                 st_a_pair(ds_tile, rl + 8 * h, jj * 8 + cq, v);
@@ -540,28 +628,20 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
             }
         }
         fence_proxy_async_smem();
-        named_bar(1 + wg, 128);                    // this warpgroup's 64 rows of the A tiles are complete
+        named_bar(1 + cw, 128);                    // this warpgroup's 64 rows of the A tiles are complete
         wgmma_fence_regs(acc0);
         if constexpr (MODE == 1) wgmma_fence_regs(acc1);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kBKV / 16; ++k) {
-            const uint64_t a0 = gmma_desc_sw128(sA + xoff + k * 32, 16, 1024);
-            const uint32_t acc_in = (it > 0 || k > 0) ? 1u : 0u;
-            if constexpr (MODE == 0) {
-                wgmma_any<NO, 0, 1>(bf16, acc0, a0, gmma_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), acc_in);
-            } else {
-                const uint64_t a1 = gmma_desc_sw128(sA + Cfg::kABytes + xoff + k * 32, 16, 1024);
-                wgmma_any<NO, 0, 1>(bf16, acc0, a0, gmma_desc_sw128(y2 + k * 2048, kBKV * 128, 1024), acc_in);
-                wgmma_any<NO, 0, 1>(bf16, acc1, a1, gmma_desc_sw128(y1 + k * 2048, kBKV * 128, 1024), acc_in);
-            }
+        const uint32_t acc_in = it > 0 ? 1u : 0u;
+        if constexpr (MODE == 0) {
+            mma_block_any<NO>(bf16, acc0, sA + xoff, y1, acc_in);
+        } else {
+            if (bf16) mma_block2<NO, true>(acc0, sA + xoff, y2, acc1, sA + Cfg::kABytes + xoff, y1, acc_in);
+            else mma_block2<NO, false>(acc0, sA + xoff, y2, acc1, sA + Cfg::kABytes + xoff, y1, acc_in);
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(acc0);
-        if constexpr (MODE == 1) wgmma_fence_regs(acc1);
-        mbar_arrive(bar_y_empty(s));
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc0);
+    if constexpr (MODE == 1) wgmma_fence_regs(acc1);
     if (MODE == 0 && p.dS) {
         // causal: key blocks past this tile's last query were never visited -- their dS is zero
         const int nblk_all = (p.n_stream + kBKV - 1) / kBKV;
@@ -597,12 +677,12 @@ cb_attention_bwd_kernel(const __grid_constant__ CUtensorMap tmX1, const __grid_c
     if constexpr (MODE == 1) store_acc(acc1, p.out2, p.ld2);
 }
 
-template <int DBOX, int MODE>
+template <int KS, int MODE>
 static int launch_attn_bwd(const CUtensorMap& x1, const CUtensorMap& x2, const CUtensorMap& y1, const CUtensorMap& y2,
                            const AttnBwdParams& p, dim3 grid, cudaStream_t st) {
-    using Cfg = AttnBwdCfg<DBOX, MODE>;
+    using Cfg = AttnBwdCfg<(KS + 3) / 4, MODE>;
     static bool done = false;
-    auto kern = cb_attention_bwd_kernel<DBOX, MODE>;
+    auto kern = cb_attention_bwd_kernel<KS, MODE>;
     if (!done) {
         CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
         done = true;
@@ -611,6 +691,22 @@ static int launch_attn_bwd(const CUtensorMap& x1, const CUtensorMap& x2, const C
     CB_CUDA(cudaGetLastError());
     count_launches(1);
     return 0;
+}
+
+// the head dim's k16 step count as a template argument: d is a multiple of 8 up to 128, so ks = ceil(d / 16) is 1..8
+template <int MODE>
+static int launch_attn_bwd_ks(int ks, const CUtensorMap& x1, const CUtensorMap& x2, const CUtensorMap& y1,
+                              const CUtensorMap& y2, const AttnBwdParams& p, dim3 grid, cudaStream_t st) {
+    switch (ks) {
+        case 1: return launch_attn_bwd<1, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 2: return launch_attn_bwd<2, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 3: return launch_attn_bwd<3, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 4: return launch_attn_bwd<4, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 5: return launch_attn_bwd<5, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 6: return launch_attn_bwd<6, MODE>(x1, x2, y1, y2, p, grid, st);
+        case 7: return launch_attn_bwd<7, MODE>(x1, x2, y1, y2, p, grid, st);
+        default: return launch_attn_bwd<8, MODE>(x1, x2, y1, y2, p, grid, st);
+    }
 }
 
 static int attn_tmap(CUtensorMap* out, int dtype, const void* ptr, long long ld, int rows, int d, int heads, int images, int box_rows) {
@@ -638,11 +734,11 @@ extern "C" int cb_attention_fwd(const void* Q, long long ldq, const void* K, lon
     AttnParams p;
     memset(&p, 0, sizeof(p));
     p.nq = nq; p.nk = nk; p.heads = heads; p.images = images;
-    p.d = d; p.dpad16 = (d + 15) / 16 * 16; p.dboxes = d <= 64 ? 1 : 2;
+    p.d = d;
     p.causal = causal;
     p.scale_log2e = scale * 1.4426950408889634f;
-    p.O = O; p.o_dtype = dtype; p.ldo = ldo; p.lse = lse;
-    p.P = P; p.ldp = ldp; p.p_is_bf16 = dtype == CB_BF16;
+    p.O = O; p.ldo = ldo; p.lse = lse;
+    p.P = P; p.ldp = ldp; p.is_bf16 = dtype == CB_BF16;
     p.two_pass = P != nullptr ? 1 : 0;
     if (P) CB_REQUIRE(ldp >= nk && ldp % 8 == 0 && (reinterpret_cast<uintptr_t>(P) & 15u) == 0, CB_ERR_ALIGN, "attention_fwd: P row pitch must be a multiple of 8 elements >= nk");
     CUtensorMap tq, tk, tv;
@@ -666,8 +762,16 @@ extern "C" int cb_attention_fwd(const void* Q, long long ldq, const void* K, lon
     }
     dim3 grid((unsigned)ceil_div(nq, kBQ), (unsigned)heads, (unsigned)images);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (p.dboxes == 1) return launch_attn<1>(tq, tk, tv, p, grid, st);
-    return launch_attn<2>(tq, tk, tv, p, grid, st);
+    switch ((d + 15) / 16) {      // k16 steps of the head dim (d is a multiple of 8 up to 128)
+        case 1: return launch_attn<1>(tq, tk, tv, p, grid, st);
+        case 2: return launch_attn<2>(tq, tk, tv, p, grid, st);
+        case 3: return launch_attn<3>(tq, tk, tv, p, grid, st);
+        case 4: return launch_attn<4>(tq, tk, tv, p, grid, st);
+        case 5: return launch_attn<5>(tq, tk, tv, p, grid, st);
+        case 6: return launch_attn<6>(tq, tk, tv, p, grid, st);
+        case 7: return launch_attn<7>(tq, tk, tv, p, grid, st);
+        default: return launch_attn<8>(tq, tk, tv, p, grid, st);
+    }
 }
 
 static int attention_bwd_impl(const void* Q, long long ldq, const void* K, long long ldk, const void* V, long long ldv,
@@ -688,7 +792,8 @@ static int attention_bwd_impl(const void* Q, long long ldq, const void* K, long 
     if (dS) CB_REQUIRE(ldds >= nk && ldds % 8 == 0 && (reinterpret_cast<uintptr_t>(dS) & 15u) == 0, CB_ERR_ALIGN, "attention_bwd: dS row pitch must be a multiple of 8 elements >= nk");
     AttnBwdParams p;
     memset(&p, 0, sizeof(p));
-    p.heads = heads; p.images = images; p.d = d; p.dpad16 = (d + 15) / 16 * 16; p.dboxes = d <= 64 ? 1 : 2;
+    p.heads = heads; p.images = images; p.d = d;
+    const int ks = (d + 15) / 16;
     p.causal = causal; p.scale = scale; p.scale_log2e = scale * 1.4426950408889634f;
     p.lse = lse; p.delta = delta; p.O = O; p.dO = dO; p.ldo = ldo; p.lddo = lddo;
     p.is_bf16 = dtype == CB_BF16; p.nq = nq;
@@ -703,7 +808,7 @@ static int attention_bwd_impl(const void* Q, long long ldq, const void* K, long 
         if ((rc = attn_tmap(&y2, dtype, V, ldv, nk, d, heads, images, kBKV))) return rc;
         p.n_stat = nq; p.n_stream = nk; p.out1 = dQ; p.ld1 = lddq; p.out2 = nullptr; p.ld2 = 0; p.dS = dS; p.ldds = ldds;
         dim3 grid((unsigned)ceil_div(nq, kBQ), (unsigned)heads, (unsigned)images);
-        rc = p.dboxes == 1 ? launch_attn_bwd<1, 0>(x1, x2, y1, y2, p, grid, st) : launch_attn_bwd<2, 0>(x1, x2, y1, y2, p, grid, st);
+        rc = launch_attn_bwd_ks<0>(ks, x1, x2, y1, y2, p, grid, st);
         if (rc) return rc;
     }
     if (run_dkdv) {
@@ -714,7 +819,7 @@ static int attention_bwd_impl(const void* Q, long long ldq, const void* K, long 
         if ((rc = attn_tmap(&y2, dtype, dO, lddo, nq, d, heads, images, kBKV))) return rc;
         p.n_stat = nk; p.n_stream = nq; p.out1 = dV; p.ld1 = lddv; p.out2 = dK; p.ld2 = lddk; p.dS = nullptr; p.ldds = 0;
         dim3 grid((unsigned)ceil_div(nk, kBQ), (unsigned)heads, (unsigned)images);
-        rc = p.dboxes == 1 ? launch_attn_bwd<1, 1>(x1, x2, y1, y2, p, grid, st) : launch_attn_bwd<2, 1>(x1, x2, y1, y2, p, grid, st);
+        rc = launch_attn_bwd_ks<1>(ks, x1, x2, y1, y2, p, grid, st);
     }
     return rc;
 }

@@ -211,12 +211,6 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// runtime fp16 / bf16 selection of the same wgmma shape
-template <int N, int TA, int TB>
-__device__ __forceinline__ void wgmma_any(bool bf16, float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-    if (bf16) Wgmma<N, true, TA, TB>::mma(d, a, b, scale_d);
-    else Wgmma<N, false, TA, TB>::mma(d, a, b, scale_d);
-}
 // named barrier over `n` threads (n a multiple of 32); ids 0..15
 __device__ __forceinline__ void named_bar(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
