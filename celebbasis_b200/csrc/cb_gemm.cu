@@ -3,7 +3,8 @@
 // One CTA computes one 128 x BN output tile:
 //   thread 0         : TMA producer (cp.async.bulk.tensor, SWIZZLE_128B boxes, mbarrier complete_tx)
 //   warpgroups 1, 2  : wgmma.mma_async on 64 rows each, fp32 accumulators in registers
-//   warpgroup 0      : epilogue (staged accumulator rows -> alpha/bias/act/residual -> HBM)
+//   warpgroup 0      : row metadata and bias row of the tile during the k-loop
+//   all 384 threads  : epilogue (staged accumulator tile -> alpha/bias/act/residual -> HBM), 8-column units
 // Convolutions never materialise im2col: each (tap, 64-channel) k-iteration loads a SHIFTED
 // [box_i][box_h][box_w][64ch] box of the NHWC image straight into the K-major A tile; padding is
 // the TMA out-of-bounds zero fill, stride-2 is the tensor-map traversal stride.
@@ -45,7 +46,6 @@ struct GemmParams {
     int d_transposed;
     int vec_ok;
     int force_stages;  // 0 auto / 3 / 6 (cb_gemm_desc.stages)
-    int vec32_ok;     // D (and R) rows are 32-byte aligned: one 32-byte sector per lane and chunk in the epilogue
     const float* bias;
     int bias_row_div;
     long long ldbias;
@@ -183,50 +183,25 @@ __device__ __forceinline__ void store8_any(void* base, int dtype, long long idx,
     else store8<__nv_bfloat16>(reinterpret_cast<__nv_bfloat16*>(base) + idx, f);
 }
 
-// Epilogue for 8 consecutive columns of one output row (one thread).  Kept deliberately small: the epilogue runs once
-// per CTA, so its cost is dominated by cold instruction fetch (~300 cycles per 128 B line of straight-line code).
-// Residual values of one 32-column chunk of this thread's row, fetched as raw 16-byte words BEFORE the accumulator is
-// needed (the loads are in flight while the MMAs / the previous chunk's stores run; D may alias R, so the compiler could
-// never hoist them itself).
-struct ResidualChunk { uint4 v[8]; };
-// one 32-byte sector as two 16-byte accesses (sm_90 has no 256-bit global load / store)
-__device__ __forceinline__ void ldg256(const void* ptr, uint4& a, uint4& b) {
-    a = reinterpret_cast<const uint4*>(ptr)[0];
-    b = reinterpret_cast<const uint4*>(ptr)[1];
-}
-__device__ __forceinline__ void stg256(void* ptr, const uint4& a, const uint4& b) {
-    reinterpret_cast<uint4*>(ptr)[0] = a;
-    reinterpret_cast<uint4*>(ptr)[1] = b;
-}
-__device__ __forceinline__ void residual_prefetch(const GemmParams& p, long long ridx, ResidualChunk& rc) {
+// Residual of one 8-column unit as raw 16-byte words (two for fp32, one for fp16 / bf16), loaded a few units before the
+// accumulator needs it.  D may alias R: every element is read and then written by the same thread, so the early load
+// never sees a value this launch stored.
+__device__ __forceinline__ void residual_load8(const GemmParams& p, long long idx, uint4 (&v)[2]) {
     if (p.r_dtype == CB_F32) {
-        const float* s = reinterpret_cast<const float*>(p.R) + ridx;
-        if (p.vec32_ok) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) ldg256(s + 8 * j, rc.v[2 * j], rc.v[2 * j + 1]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) rc.v[j] = reinterpret_cast<const uint4*>(s)[j];
-        }
+        const uint4* s = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.R) + idx);
+        v[0] = s[0];
+        v[1] = s[1];
     } else {
-        const __half* s = reinterpret_cast<const __half*>(p.R) + ridx;
-        if (p.vec32_ok) {
-#pragma unroll
-            for (int j = 0; j < 2; ++j) ldg256(s + 16 * j, rc.v[2 * j], rc.v[2 * j + 1]);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) rc.v[j] = reinterpret_cast<const uint4*>(s)[j];
-        }
+        v[0] = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(p.R) + idx);
     }
 }
-__device__ __forceinline__ void residual_unpack8(const GemmParams& p, const ResidualChunk& rc, int g, float (&r)[8]) {
+__device__ __forceinline__ void residual_unpack8(const GemmParams& p, const uint4 (&v)[2], float (&r)[8]) {
     if (p.r_dtype == CB_F32) {
-        const uint4 a = rc.v[2 * g], b = rc.v[2 * g + 1];
+        const uint4 a = v[0], b = v[1];
         r[0] = __uint_as_float(a.x); r[1] = __uint_as_float(a.y); r[2] = __uint_as_float(a.z); r[3] = __uint_as_float(a.w);
         r[4] = __uint_as_float(b.x); r[5] = __uint_as_float(b.y); r[6] = __uint_as_float(b.z); r[7] = __uint_as_float(b.w);
     } else {
-        const uint4 a = rc.v[g];
-        const uint32_t w[4] = {a.x, a.y, a.z, a.w};
+        const uint32_t w[4] = {v[0].x, v[0].y, v[0].z, v[0].w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             float2 t;
@@ -237,9 +212,9 @@ __device__ __forceinline__ void residual_unpack8(const GemmParams& p, const Resi
     }
 }
 
-// kExt: the instantiation that carries the rarely used epilogue features (second destination, PReLU slopes, D2 affine).
-// They are compiled OUT of the common instantiation: the epilogue runs once per CTA and its cost is cold instruction
-// fetch, so every extra line of straight-line code is paid by all 700+ GEMM launches of the step.
+// Epilogue of one 8-column unit of one output row: alpha is applied by the caller; bias, activation, residual, store D,
+// then D2 with its affine.  kExt is the instantiation that carries the rarely used features (second destination, PReLU
+// slopes, D2 affine, GEGLU), so the common instantiation does not carry their code.
 template <bool kExt>
 __device__ __forceinline__ void epilogue_group8(const GemmParams& p, float (&f)[8], long long grow, long long brow, int col,
                                              long long d_off, long long r_off, int ncols, const float* rpre = nullptr,
@@ -248,7 +223,7 @@ __device__ __forceinline__ void epilogue_group8(const GemmParams& p, float (&f)[
 #pragma unroll
         for (int j = 0; j < 8; ++j) f[j] += sbias[j];
     } else if (p.bias) {
-        if (ncols == 8) {
+        if (ncols == 8 && p.vec_ok) {      // vec_ok: 16-byte aligned bias rows
             float b[8];
             load8<float>(p.bias + brow * p.ldbias + col, b);
 #pragma unroll
@@ -304,143 +279,22 @@ __device__ __forceinline__ void epilogue_group8(const GemmParams& p, float (&f)[
     }
 }
 
-// GEGLU (attention.py:37-45) inside the FF-in projection's epilogue.  The weight rows are interleaved at load time so that
-// every 64-column group of the GEMM output holds 32 value columns followed by their 32 gate columns; this thread's row of
-// such a group arrives as two accumulator chunks.  D (optional) keeps the pre-activations for the backward pass, D2
-// receives value * gelu(gate) at column (group * 32).
-__device__ __forceinline__ void epilogue_glu64(const GemmParams& p, float (&fv)[32], float (&fg)[32], long long grow, int col,
-                                               const float* sbias) {
-    uint4 pk[4];
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-        float(&f)[32] = half ? fg : fv;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-            float b[8];
-            if (sbias) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) b[j] = sbias[half * 32 + g * 8 + j];
-            } else if (p.bias) {
-                load8<float>(p.bias + col + half * 32 + g * 8, b);
-            } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) b[j] = 0.f;
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[g * 8 + j] += b[j];
-            if (p.D) {
-                float t[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) t[j] = f[g * 8 + j];
-                store8_any(p.D, p.d_dtype, grow * p.ldd + col + half * 32 + g * 8, t);
-            }
-        }
-    }
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-        float u[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) u[j] = fv[g * 8 + j] * gelu_f(fg[g * 8 + j]);
-        store8_any(p.D2, p.d2_dtype, grow * p.ldd2 + (col >> 1) + g * 8, u);
-    }
-    (void)pk;
-}
-
-// Full 32-column chunk of one output row on the aligned fast path: bias / activation / residual on registers, then
-// 256-bit stores (one full 32-byte sector per lane and instruction) when the rows are 32-byte aligned.
-template <bool kExt>
-__device__ __forceinline__ void epilogue_chunk32(const GemmParams& p, const float (&fin)[32], long long grow, long long brow,
-                                                 int col, long long d_off, long long r_off, const ResidualChunk* rc,
-                                                 const float* sbias) {
-    const long long didx = d_off + grow * p.ldd + col;
-    uint4 pk[4];
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-        float f[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = fin[g * 8 + j];
-        if (sbias) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] += sbias[g * 8 + j];
-        } else if (p.bias) {
-            float b[8];
-            load8<float>(p.bias + brow * p.ldbias + col + g * 8, b);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] += b[j];
-        }
-        if (p.act != CB_ACT_NONE) {
-            if constexpr (kExt) {
-                apply_act8(f, p.act, p.act_param, col + g * 8);
-            } else {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) f[j] = apply_act(f[j], p.act);
-            }
-        }
-        if (rc) {
-            float r[8];
-            residual_unpack8(p, *rc, g, r);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] += r[j];
-        } else if (p.R) {
-            float r[8];
-            const long long ridx = r_off + grow * p.ldr + col + g * 8;
-            if (p.r_dtype == CB_F32) load8<float>(reinterpret_cast<const float*>(p.R) + ridx, r);
-            else if (p.r_dtype == CB_F16) load8<__half>(reinterpret_cast<const __half*>(p.R) + ridx, r);
-            else load8<__nv_bfloat16>(reinterpret_cast<const __nv_bfloat16*>(p.R) + ridx, r);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) f[j] += r[j];
-        }
-        if constexpr (kExt) {
-            if (p.D2) {
-                float g2[8];
-                d2_affine8(g2, f, p.d2_scale, p.d2_shift, col + g * 8);
-                store8_any(p.D2, p.d2_dtype, grow * p.ldd2 + col + g * 8, g2);
-            }
-        }
-        if (p.d_dtype == CB_F32) {
-            float* dst = reinterpret_cast<float*>(p.D) + didx + g * 8;
-            const uint4 a = make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
-            const uint4 b = make_uint4(__float_as_uint(f[4]), __float_as_uint(f[5]), __float_as_uint(f[6]), __float_as_uint(f[7]));
-            if (p.vec32_ok) stg256(dst, a, b);
-            else { reinterpret_cast<uint4*>(dst)[0] = a; reinterpret_cast<uint4*>(dst)[1] = b; }
-        } else {
-            if (p.d_dtype == CB_F16) {
-                __half2* h = reinterpret_cast<__half2*>(&pk[g]);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(f[2 * i], f[2 * i + 1]);
-            } else {
-                __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&pk[g]);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-            }
-            if (g & 1) {
-                uint16_t* dst = reinterpret_cast<uint16_t*>(p.D) + didx + (g - 1) * 8;
-                if (p.vec32_ok) stg256(dst, pk[g - 1], pk[g]);
-                else { reinterpret_cast<uint4*>(dst)[0] = pk[g - 1]; reinterpret_cast<uint4*>(dst)[1] = pk[g]; }
-            }
-        }
-    }
-}
-
 // Warp roles (384 threads, one CTA per SM):
-//   warpgroup 0 : thread 0 is the TMA producer; after the main loop all 128 threads run the epilogue, one output row each
+//   warpgroup 0 : thread 0 is the TMA producer; the other threads stage the tile's row metadata and bias row meanwhile
 //   warpgroups 1, 2 : wgmma consumers, rows [0, 64) and [64, 128) of the tile, fp32 accumulators in registers
 // Once the last k-iteration has retired, the consumers park their accumulators in the (then idle) TMA ring as a row-major
-// fp32 tile of pitch BN + 4 floats (conflict-free 16-byte row reads), so the epilogue reads one row per thread.
+// fp32 tile of pitch BN + 4 floats, and all 384 threads run the epilogue on it (epilogue_units).
 template <int BN>
 struct StageCfg {
     static constexpr int kPitch = BN + 4;
     static constexpr int kBytes = ((BM * kPitch * 4) + 1023) / 1024 * 1024;
 };
 
-// 32 consecutive accumulator columns of this thread's row from the staged tile
-__device__ __forceinline__ void stage_ld32(const float* row, int c, uint32_t (&acc)[32]) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        const float4 v = *reinterpret_cast<const float4*>(row + c * 32 + 4 * j);
-        acc[4 * j] = __float_as_uint(v.x); acc[4 * j + 1] = __float_as_uint(v.y);
-        acc[4 * j + 2] = __float_as_uint(v.z); acc[4 * j + 3] = __float_as_uint(v.w);
-    }
+// 8 consecutive accumulator columns of the staged tile, times alpha
+__device__ __forceinline__ void stage_ld8(const float* src, float alpha, float (&f)[8]) {
+    const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
+    f[0] = a.x * alpha; f[1] = a.y * alpha; f[2] = a.z * alpha; f[3] = a.w * alpha;
+    f[4] = b.x * alpha; f[5] = b.y * alpha; f[6] = b.z * alpha; f[7] = b.w * alpha;
 }
 
 // ---- split-K hand-off through L2 (all 384 threads): every CTA stores its fp32 partial tile into its own slice of the
@@ -533,6 +387,136 @@ __device__ __forceinline__ void mma_kiter(float (&acc)[BN / 2], uint32_t a_src, 
     }
 }
 
+// ---- epilogue, all 384 threads.  The work unit is 8 consecutive columns of one row of the staged fp32 tile
+//      (epilogue_group8).  Unit u of the tile is row u / (BN / 8), column group u % (BN / 8), so the lanes of a warp cover
+//      consecutive column groups of the same rows: every D / D2 store and residual load of a warp writes or reads whole
+//      rows of the tile (two rows per warp at BN = 128, four at BN = 64).  Thread t takes units t, t + 384, ...
+//      - transposed D: unit u is row u % 128 of column group u / 128, so the lanes store consecutive rows of one column;
+//      - GEGLU: the unit is one 8-column slice of the 32 value columns of a 64-column group and the matching 8 gate columns;
+//      - the residual of a thread's next kResAhead units is in flight while it works on the current one;
+//      - cluster split-K: every thread sends units of its partial tile to their owner CTAs, then sums the units it owns
+//        over the senders in sender order 0..S-1 and finishes them like the ordinary path.  Both phases map the lanes to
+//        consecutive rows of one group, so the exchange slots a warp writes and reads are contiguous.
+template <int BN, bool kExt>
+__device__ __forceinline__ void epilogue_units(const GemmParams& p, const float* stage, const long long* s_grow,
+                                               const int* s_brow, const float* s_bias, int n0, int ncols_tile, int zo,
+                                               int zi, int sp, uint32_t xbuf, unsigned long long* dbg) {
+    constexpr int kPitch = StageCfg<BN>::kPitch;
+    constexpr int G = BN / 8;             // column groups per tile row
+    constexpr int kResAhead = 2;
+    const long long d_off = (long long)zo * p.d_bs2 + (long long)zi * p.d_bs;
+    const long long r_off = (long long)zo * p.r_bs2 + (long long)zi * p.r_bs;
+    const int tid = threadIdx.x;
+    auto sbias_of = [&](int row, int col) { return p.bias && s_brow[row] < 0 ? s_bias + col : nullptr; };
+
+    if (p.cluster_sk) {
+        const int S = p.splits;
+        const int GI = (G + S - 1) / S;                      // groups a CTA can own: group g -> CTA g % S
+        fence_proxy_async_smem();                            // the ring was written / read through the async proxy
+        cluster_sync_all();                                  // #1: every CTA of the cluster has staged its accumulator
+        for (int u = tid; u < BM * G; u += kThreads) {
+            const int row = u % BM, g = u / BM;              // lanes: consecutive rows, i.e. consecutive 32-byte slots
+            if (g * 8 < ncols_tile) {
+                const float* src = stage + row * kPitch + g * 8;
+                const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
+                const uint32_t v[8] = {__float_as_uint(a.x), __float_as_uint(a.y), __float_as_uint(a.z), __float_as_uint(a.w),
+                                       __float_as_uint(b.x), __float_as_uint(b.y), __float_as_uint(b.z), __float_as_uint(b.w)};
+                st_cluster_f32x8(xbuf + static_cast<uint32_t>(((sp * GI + g / S) * BM + row) * 32), static_cast<uint32_t>(g % S), v);
+            }
+        }
+        cluster_sync_all();                                  // #2: all partial groups have landed in their owners
+#pragma unroll 1
+        for (int u = tid; u < BM * GI; u += kThreads) {
+            const int row = u % BM, gi = u / BM;             // an owner's groups are S apart: no row-contiguous stores
+            const int g = gi * S + sp;
+            const long long grow = s_grow[row];
+            if (g * 8 >= ncols_tile || grow < 0) continue;
+            float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+            for (int s2 = 0; s2 < S; ++s2) {
+                const uint32_t a = xbuf + static_cast<uint32_t>(((s2 * GI + gi) * BM + row) * 32);
+                const float4 lo = ld_shared_f32x4(a), hi = ld_shared_f32x4(a + 16);
+                f[0] += lo.x; f[1] += lo.y; f[2] += lo.z; f[3] += lo.w;
+                f[4] += hi.x; f[5] += hi.y; f[6] += hi.z; f[7] += hi.w;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) f[j] *= p.alpha;
+            epilogue_group8<kExt>(p, f, grow, s_brow[row], n0 + g * 8, d_off, r_off, min(8, ncols_tile - g * 8), nullptr,
+                                  sbias_of(row, g * 8));
+        }
+        return;
+    }
+
+    if constexpr (kExt) {
+        if (p.glu) {
+            // column group c64 of the tile holds 32 value columns, then their 32 gate columns (N % 64 == 0, no per-image
+            // bias: the bias row is always the staged one)
+            constexpr int GQ = BN / 16;
+#pragma unroll 1
+            for (int u = tid; u < BM * GQ; u += kThreads) {
+                const int row = u / GQ, q = u % GQ;
+                const int vcol = (q >> 2) * 64 + (q & 3) * 8;
+                const long long grow = s_grow[row];
+                if (vcol >= ncols_tile || grow < 0) continue;
+                float fv[8], fg[8];
+                stage_ld8(stage + row * kPitch + vcol, p.alpha, fv);
+                stage_ld8(stage + row * kPitch + vcol + 32, p.alpha, fg);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    fv[j] += p.bias ? s_bias[vcol + j] : 0.f;
+                    fg[j] += p.bias ? s_bias[vcol + 32 + j] : 0.f;
+                }
+                if (p.D) {
+                    store8_any(p.D, p.d_dtype, grow * p.ldd + n0 + vcol, fv);
+                    store8_any(p.D, p.d_dtype, grow * p.ldd + n0 + vcol + 32, fg);
+                }
+                float h[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) h[j] = fv[j] * gelu_f(fg[j]);
+                store8_any(p.D2, p.d2_dtype, grow * p.ldd2 + ((n0 + (q >> 2) * 64) >> 1) + (q & 3) * 8, h);
+            }
+            return;
+        }
+    }
+
+    // residual fast path (whole aligned units of a row-major D): raw residual of this thread's units k .. k + kResAhead
+    const bool r_pre = p.R && p.vec_ok && !p.d_transposed;
+    uint4 rq[kResAhead + 1][2];
+    auto res_fetch = [&](int k, uint4 (&v)[2]) {
+        const int u = tid + k * kThreads;
+        if (u >= BM * G) return;
+        const int row = u / G, col = (u % G) * 8;
+        const long long grow = s_grow[row];
+        if (grow >= 0 && col + 8 <= ncols_tile) residual_load8(p, r_off + grow * p.ldr + n0 + col, v);
+    };
+    if (r_pre) {
+#pragma unroll
+        for (int k = 0; k < kResAhead; ++k) res_fetch(k, rq[k]);
+    }
+    const int nunits = (BM * G - tid + kThreads - 1) / kThreads;
+#pragma unroll 1
+    for (int k = 0; k < nunits; ++k) {
+        if (r_pre) res_fetch(k + kResAhead, rq[kResAhead]);
+        const int u = tid + k * kThreads;
+        const int row = p.d_transposed ? u % BM : u / G;
+        const int col = (p.d_transposed ? u / BM : u % G) * 8;
+        const long long grow = s_grow[row];
+        if (col < ncols_tile && grow >= 0) {
+            const int ncols = min(8, ncols_tile - col);
+            float f[8], r[8];
+            stage_ld8(stage + row * kPitch + col, p.alpha, f);
+            if (r_pre && ncols == 8) residual_unpack8(p, rq[0], r);
+            epilogue_group8<kExt>(p, f, grow, s_brow[row], n0 + col, d_off, r_off, ncols, r_pre && ncols == 8 ? r : nullptr,
+                                  sbias_of(row, col));
+        }
+        if (dbg && k == 0 && tid == 64) dbg[6] = clock64();
+        if (r_pre) {
+#pragma unroll
+            for (int j = 0; j < kResAhead; ++j) { rq[j][0] = rq[j + 1][0]; rq[j][1] = rq[j + 1][1]; }
+        }
+    }
+}
+
 template <int BN, bool A_MN, bool B_MN, int kStages, bool kExt>
 __global__ void __launch_bounds__(kThreads, 1)
 cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -546,6 +530,9 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
 
+    __shared__ long long s_grow[BM];           // global output row of each tile row, -1 past the edge of D
+    __shared__ int s_brow[BM];                 // bias row of each tile row, -1 for the tile's first (staged) one
+    __shared__ __align__(16) float s_bias[BN];
     const int warp = threadIdx.x >> 5;
     // warp-uniform as far as the compiler can tell: with a plain threadIdx-derived index the consumer branch counts as
     // divergent, and ptxas serialises every wgmma.mma_async in it (C7520), waiting for each MMA before issuing the next
@@ -634,6 +621,33 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
         }
         __syncwarp();
+        // while the consumers run the k-loop: global row (or -1 past the edge) and bias row of every tile row, and the bias
+        // row of the tile's first output row in shared memory.  Conv tiles are [box_i][box_h][box_w] pixel boxes.
+        const int r = threadIdx.x;
+        long long grow;
+        bool row_valid;
+        if (p.conv) {
+            const int per_img = p.box_h * p.box_w;
+            const int bi = r / per_img;
+            const int rem = r - bi * per_img;
+            const int bh = rem / p.box_w;
+            const int bw = rem - bh * p.box_w;
+            const int img = img0 + bi, oh = oh0 + bh, ow = ow0 + bw;
+            row_valid = (bi < p.box_i) && (img < p.img_n) && (oh < p.out_h) && (ow < p.out_w);
+            grow = ((long long)img * p.out_h + oh) * p.out_w + ow;
+        } else {
+            grow = m0 + r;
+            row_valid = grow < p.M;
+        }
+        s_grow[r] = row_valid ? grow : -1;
+        if (p.bias) {
+            const long long tile_row0 = p.conv ? (((long long)img0 * p.out_h + oh0) * p.out_w + ow0) : (long long)m0;
+            const long long brow0 = p.bias_row_div > 0 ? tile_row0 / p.bias_row_div : 0;
+            const long long brow = p.bias_row_div > 0 ? grow / p.bias_row_div : 0;
+            s_brow[r] = brow == brow0 ? -1 : static_cast<int>(brow);
+            const int ncols = min(BN, p.N - n0);
+            for (int i = r; i < BN; i += 128) s_bias[i] = i < ncols ? p.bias[brow0 * p.ldbias + n0 + i] : 0.f;
+        }
     } else {
         // ===================== wgmma consumers =====================
         float acc[BN / 2];
@@ -675,142 +689,16 @@ cb_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             *reinterpret_cast<float2*>(srow + 8 * SCfg::kPitch + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
     }
-    named_bar(2, kThreads);        // accumulator tile staged
-    if (p.cluster_sk && wg != 0) { cluster_sync_all(); cluster_sync_all(); }   // the two cluster barriers of the epilogue
+    named_bar(2, kThreads);        // accumulator tile, row metadata and bias row staged
     const int ncols_tile = min(BN, p.N - n0);
     if (p.splits > 1 && !p.cluster_sk && p.dbg_mode == 0) {
         const unsigned tile_id = (static_cast<unsigned>(bz) * gridDim.y + m_tile) * gridDim.x + blockIdx.x;
         if (!splitk_reduce_to_stage<BN>(p, tile_id, sp, stage, ncols_tile)) return;
     }
-
-    if (wg == 0) {
-        // ===================== epilogue: one output row per thread =====================
-        const int r = threadIdx.x;
-        bool row_valid;
-        long long grow;
-        if (p.conv) {
-            const int per_img = p.box_h * p.box_w;
-            const int bi = r / per_img;
-            const int rem = r - bi * per_img;
-            const int bh = rem / p.box_w;
-            const int bw = rem - bh * p.box_w;
-            const int img = img0 + bi, oh = oh0 + bh, ow = ow0 + bw;
-            row_valid = (bi < p.box_i) && (img < p.img_n) && (oh < p.out_h) && (ow < p.out_w);
-            grow = ((long long)img * p.out_h + oh) * p.out_w + ow;
-        } else {
-            grow = m0 + r;
-            row_valid = grow < p.M;
-        }
-        const long long brow = p.bias_row_div > 0 ? grow / p.bias_row_div : 0;
-        const long long d_off = (long long)zo * p.d_bs2 + (long long)zi * p.d_bs;
-        const long long r_off = (long long)zo * p.r_bs2 + (long long)zi * p.r_bs;
-        // bias row of this tile -> shared memory (global bias loads in the store loop would each wait a full L2 round
-        // trip behind the previous chunk's stores)
-        __shared__ __align__(16) float s_bias[BN + 8];
-        const float* sb = nullptr;
-        if (p.bias) {
-            const long long tile_row0 = p.conv ? (((long long)img0 * p.out_h + oh0) * p.out_w + ow0) : (long long)m0;
-            const long long brow0 = p.bias_row_div > 0 ? tile_row0 / p.bias_row_div : 0;
-            for (int i = threadIdx.x; i < BN; i += 128) s_bias[i] = i < ncols_tile ? p.bias[brow0 * p.ldbias + n0 + i] : 0.f;
-            named_bar(3, 128);
-            if (brow == brow0) sb = s_bias;
-        }
-        // residual fast path: whole 32-column chunks, 16-byte aligned rows
-        const bool r_fast = p.R && p.vec_ok && !p.d_transposed && row_valid;
-        const long long r_row = r_off + grow * p.ldr + n0;
-        ResidualChunk rc_cur, rc_next;
-        if (r_fast && ncols_tile >= 32) residual_prefetch(p, r_row, rc_cur);
-        if (dbg && threadIdx.x == 64) dbg[4] = clock64();
-        const float* trow = stage + r * SCfg::kPitch;
-        if (p.dbg_mode == 1 || p.dbg_mode == 2) {
-        } else if (!p.cluster_sk) {     // one k-slice, or the sum of the k-slices (splitk_reduce_to_stage)
-#pragma unroll 1
-            for (int c = 0; c * 32 < ncols_tile; ++c) {
-                uint32_t acc[32];
-                if constexpr (kExt) {
-                    if (p.glu) {
-                        uint32_t acc2[32];
-                        stage_ld32(trow, c, acc);
-                        stage_ld32(trow, c + 1, acc2);
-                        if (row_valid) {
-                            float fv[32], fg[32];
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) { fv[j] = __uint_as_float(acc[j]) * p.alpha; fg[j] = __uint_as_float(acc2[j]) * p.alpha; }
-                            epilogue_glu64(p, fv, fg, grow, n0 + c * 32, sb ? sb + c * 32 : nullptr);
-                        }
-                        ++c;
-                        continue;
-                    }
-                }
-                stage_ld32(trow, c, acc);
-                const bool pre = r_fast && ncols_tile - c * 32 >= 32;
-                if (r_fast && ncols_tile - (c + 1) * 32 >= 32) residual_prefetch(p, r_row + (c + 1) * 32, rc_next);
-                if (row_valid && p.vec_ok && !p.d_transposed && ncols_tile - c * 32 >= 32) {
-                    float f[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(acc[j]) * p.alpha;
-                    epilogue_chunk32<kExt>(p, f, grow, brow, n0 + c * 32, d_off, r_off, pre ? &rc_cur : nullptr, sb ? sb + c * 32 : nullptr);
-                } else if (row_valid) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const int nc = min(8, ncols_tile - c * 32 - g * 8);
-                        if (nc > 0) {
-                            float f[8];
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(acc[g * 8 + j]) * p.alpha;
-                            epilogue_group8<kExt>(p, f, grow, brow, n0 + c * 32 + g * 8, d_off, r_off, nc, nullptr, sb ? sb + c * 32 + g * 8 : nullptr);
-                        }
-                    }
-                }
-                rc_cur = rc_next;
-            }
-        } else {
-            // ---- split-K inside a thread-block cluster: the `splits` CTAs of this tile are the cluster (1,1,splits), rank =
-            //      k-slice.  The 8-column groups of the tile are dealt round-robin to the CTAs (group g -> CTA g % S); every CTA
-            //      sends each group of its partial accumulator into the owner's exchange buffer (the part of the idle TMA ring
-            //      behind the staged tile), slot [sender][g / S][row] of 32 bytes, then sums its own groups over the S senders
-            //      and runs the epilogue for them.  Two cluster barriers replace the L2 reductions, the __threadfence, the
-            //      arrival counter and the read-back of the global-workspace path.
-            const int S = p.splits;
-            const int GI = (BN / 8 + S - 1) / S;                 // groups a CTA can own
-            const uint32_t xbuf = smem_base + SCfg::kBytes;
-            fence_proxy_async_smem();                            // the ring was written / read through the async proxy
-            cluster_sync_all();                                  // #1: every CTA of the cluster has staged its accumulator
-#pragma unroll 1
-            for (int c = 0; c * 32 < ncols_tile; ++c) {
-                uint32_t acc[32];
-                stage_ld32(trow, c, acc);
-#pragma unroll
-                for (int gq = 0; gq < 4; ++gq) {
-                    const int g = c * 4 + gq;
-                    if (g * 8 < ncols_tile)
-                        st_cluster_f32x8(xbuf + static_cast<uint32_t>(((sp * GI + g / S) * BM + r) * 32),
-                                         static_cast<uint32_t>(g % S), &acc[gq * 8]);
-                }
-            }
-            cluster_sync_all();                                  // #2: all partial groups have landed in their owners
-            for (int gi = 0; gi < GI; ++gi) {
-                const int g = gi * S + sp;
-                if (g * 8 >= ncols_tile) break;
-                float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll 4
-                for (int s2 = 0; s2 < S; ++s2) {
-                    const uint32_t a = xbuf + static_cast<uint32_t>(((s2 * GI + gi) * BM + r) * 32);
-                    const float4 lo = ld_shared_f32x4(a), hi = ld_shared_f32x4(a + 16);
-                    f[0] += lo.x; f[1] += lo.y; f[2] += lo.z; f[3] += lo.w;
-                    f[4] += hi.x; f[5] += hi.y; f[6] += hi.z; f[7] += hi.w;
-                }
-                if (row_valid) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) f[j] *= p.alpha;
-                    epilogue_group8<kExt>(p, f, grow, brow, n0 + g * 8, d_off, r_off, min(8, ncols_tile - g * 8), nullptr,
-                                          sb ? sb + g * 8 : nullptr);
-                }
-            }
-        }
-        if (dbg && threadIdx.x == 64) dbg[5] = clock64();
-    }
-    if (dbg && threadIdx.x == 0) dbg[6] = clock64();
+    if (p.dbg_mode == 1 || p.dbg_mode == 2) return;
+    if (dbg && threadIdx.x == 64) dbg[4] = clock64();
+    epilogue_units<BN, kExt>(p, stage, s_grow, s_brow, s_bias, n0, ncols_tile, zo, zi, sp, smem_base + SCfg::kBytes, dbg);
+    if (dbg && threadIdx.x == 64) dbg[5] = clock64();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1141,14 +1029,6 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
         }
         if (d.bias) ok = ok && ((reinterpret_cast<uintptr_t>(d.bias) & 15u) == 0) && ((d.ldbias * 4) % 16 == 0);
         p.vec_ok = ok ? 1 : 0;
-        bool ok32 = ok && ((reinterpret_cast<uintptr_t>(d.D) & 31u) == 0) && ((d.ldd * des) % 32 == 0) &&
-                    ((d.d_batch_stride * des) % 32 == 0) && ((d.d_batch_stride2 * des) % 32 == 0);
-        if (d.R) {
-            const int res = d.r_dtype == CB_F32 ? 4 : 2;
-            ok32 = ok32 && ((reinterpret_cast<uintptr_t>(d.R) & 31u) == 0) && ((d.ldr * res) % 32 == 0) &&
-                   ((d.r_batch_stride * res) % 32 == 0) && ((d.r_batch_stride2 * res) % 32 == 0);
-        }
-        p.vec32_ok = ok32 ? 1 : 0;
     }
 
     // ---- split-K heuristic: fill the SMs when the tile grid alone cannot (bs=1 low-resolution layers) ----

@@ -23,8 +23,8 @@ def report(name, fn, ncta_max=4096):
     g0 = t[:, 7].min()
     print(f"{name}: ctas={t.shape[0]} cta_start_spread={(t[:, 7].max() - g0) / 1000:.2f}us | per-CTA (SM clock @1.965GHz, mean/max us): "
           f"setup={d(0,1).mean():.2f} first_full={d(1,2).mean():.2f} mainloop_issue={d(2,3).mean():.2f}/{d(2,3).max():.2f} "
-          f"mma_drain={d(3,4).mean():.2f} epilogue={d(4,5).mean():.2f}/{d(4,5).max():.2f} tail_sync={d(5,6).mean():.2f} "
-          f"total={d(0,6).mean():.2f}/{d(0,6).max():.2f}")
+          f"mma_drain={d(3,4).mean():.2f} epilogue={d(4,5).mean():.2f}/{d(4,5).max():.2f} first_unit={d(4,6).mean():.2f} "
+          f"total={d(0,5).mean():.2f}/{d(0,5).max():.2f}")
 
 
 def conv(n, h, cin, cout):
