@@ -5,8 +5,13 @@
 // the nn.SiLU that follows them in ResBlock (openaimodel.py:201-241) and nn.LayerNorm in
 // BasicTransformerBlock (attention.py:196-215) / CLIP layers.  HBM-bound: every kernel reads its
 // input once (2-wide / 4-wide vector loads, channel index fastest => fully coalesced rows) and the
-// statistics pass keeps per-thread partials in registers, one shared atomic per channel pair and one
-// fp64 global atomic per (block, group).
+// statistics pass keeps per-thread partials in registers, adds them per group in a fixed order in
+// shared memory, and combines the CTAs' (sum, sumsq) partials in a fixed order: through distributed
+// shared memory inside a thread-block cluster, or as one partial per (CTA, group) in the workspace
+// that the apply kernel adds up in CTA order.
+//
+// GroupNorm dispatch: forward = cluster kernel where the rows fit in shared memory, else the TMA-streamed
+// statistics + apply pair; backward = cluster kernel, else the statistics + apply pair.
 #include "cb_common.cuh"
 
 namespace cb {
@@ -95,7 +100,7 @@ __device__ __forceinline__ void group_acc_flush(float* s_a, float* s_b, int n) {
     }
     __syncthreads();
 }
-// streaming two-kernel path: the statistics kernel publishes one (sum, sum2) partial per CTA and group, the apply kernel
+// statistics + apply kernel pairs: the statistics kernel publishes one (sum, sum2) partial per CTA and group, the apply kernel
 // (same grid) adds them up in CTA order
 __device__ __forceinline__ void publish_block_partials(double* ws, const float* s_a, const float* s_b, int G) {
     if ((int)threadIdx.x < G)
@@ -115,10 +120,9 @@ __device__ __forceinline__ double2 sum_block_partials(const double* ws, int G, i
 
 constexpr int kGnMaxDynSmem = 184 * 1024;  // dynamic shared memory of the staged variants (+ GnSlots + statics <= 227 KiB)
 constexpr int kGnThreads = 256;           // upper bound; the launch uses PW*RY threads (see gn_shape)
-constexpr int kGnFusedThreads = 1024;     // fused kernels: one CTA per SM, so fill it (PW x up-to-1024/PW row lanes)
 constexpr int kGnMaxChunks = 8;           // channel-pair chunks per thread: C <= 2*PW*8
 
-// Thread mapping shared by the four GroupNorm kernels: a block is a (RY x PW) grid of threads; tx owns channel
+// Thread mapping shared by the statistics + apply GroupNorm kernels: a block is a (RY x PW) grid of threads; tx owns channel
 // pairs {tx + j*PW}, ty strides over the rows of the block's row range.  PW is the largest divisor of C/2 that is
 // <= 256, so every thread is busy for C = 128 (PW 64, RY 4) as well as C = 320 (PW 160, RY 1) or C = 2560 (PW 256).
 struct GnShape { int pw, ry, chunks; };
@@ -133,100 +137,9 @@ static inline GnShape gn_shape(int C) {
     return s;
 }
 
-// ---- GroupNorm statistics: one (sum, sumsq) partial per CTA and group into ws (publish_block_partials) ----------
-template <typename TX>
-__global__ void __launch_bounds__(kGnThreads)
-gn_stats_kernel(const TX* __restrict__ x, double* __restrict__ ws, int HW, int C, int G, int rows_per_block, int PW,
-                int RY, int chunks) {
-    pdl_sync();
-    __shared__ float s_sum[64], s_sq[64];
-    const int n = blockIdx.y;
-    const int tx = threadIdx.x % PW, ty = threadIdx.x / PW;
-    const int r0 = blockIdx.x * rows_per_block;
-    const int r1 = min(HW, r0 + rows_per_block);
-    const int cpg = C / G;
-    if (threadIdx.x < 64) { s_sum[threadIdx.x] = 0.f; s_sq[threadIdx.x] = 0.f; }
-    group_acc_begin();
-    __syncthreads();
-    float a1[kGnMaxChunks], a2[kGnMaxChunks];
-#pragma unroll
-    for (int j = 0; j < kGnMaxChunks; ++j) { a1[j] = 0.f; a2[j] = 0.f; }
-    const TX* xb = x + ((size_t)n * HW) * C + 2 * tx;
-#pragma unroll 8
-    for (int r = r0 + ty; r < r1; r += RY) {
-        const TX* xr = xb + (size_t)r * C;
-#pragma unroll
-        for (int j = 0; j < kGnMaxChunks; ++j) {
-            if (j < chunks) {
-                const float2 v = Vec2<TX>::ld(xr + 2 * j * PW);
-                a1[j] += v.x + v.y;
-                a2[j] += v.x * v.x + v.y * v.y;
-            }
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < kGnMaxChunks; ++j) {
-        if (j < chunks) {
-            const int g = (2 * (tx + j * PW)) / cpg;
-            group_accumulate(s_sum, s_sq, g, a1[j], a2[j]);
-        }
-    }
-    __syncthreads();
-    group_acc_flush(s_sum, s_sq, 64);
-    publish_block_partials(ws, s_sum, s_sq, G);
-}
-
-// ---- GroupNorm apply: y = act((x-mean)*rstd*gamma+beta) ---------------------------------------------
-template <typename TX, typename TY>
-__global__ void __launch_bounds__(kGnThreads)
-gn_apply_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* __restrict__ gamma,
-                const float* __restrict__ beta, const double* __restrict__ ws, float* __restrict__ mean_out,
-                float* __restrict__ rstd_out, int HW, int C, int G, float eps, int act, int rows_per_block, int PW,
-                int RY, int chunks) {
-    pdl_sync();
-    __shared__ float s_mean[64], s_rstd[64];
-    const int n = blockIdx.y;
-    const int tx = threadIdx.x % PW, ty = threadIdx.x / PW;
-    const int cpg = C / G;
-    if (threadIdx.x < G) {
-        const double cnt = (double)HW * cpg;
-        const double2 sums = sum_block_partials(ws, G, threadIdx.x);
-        const double m = sums.x / cnt;
-        double var = sums.y / cnt - m * m;
-        if (var < 0) var = 0;
-        const float rs = (float)(1.0 / sqrt(var + (double)eps));
-        s_mean[threadIdx.x] = (float)m;
-        s_rstd[threadIdx.x] = rs;
-        if (blockIdx.x == 0) {
-            mean_out[n * G + threadIdx.x] = (float)m;
-            rstd_out[n * G + threadIdx.x] = rs;
-        }
-    }
-    __syncthreads();
-    const int r0 = blockIdx.x * rows_per_block;
-    const int r1 = min(HW, r0 + rows_per_block);
-    const size_t base = ((size_t)n * HW) * C;
-    for (int j = 0; j < chunks; ++j) {
-        const int c = 2 * (tx + j * PW);
-        const int g = c / cpg;
-        const float m = s_mean[g], rs = s_rstd[g];
-        const float g0 = gamma[c] * rs, g1 = gamma[c + 1] * rs;
-        const float b0 = beta[c] - m * g0, b1 = beta[c + 1] - m * g1;
-#pragma unroll 8
-        for (int r = r0 + ty; r < r1; r += RY) {
-            const size_t off = base + (size_t)r * C + c;
-            float2 v = Vec2<TX>::ld(x + off);
-            v.x = v.x * g0 + b0;
-            v.y = v.y * g1 + b1;
-            if (act) { v.x = silu_f(v.x); v.y = silu_f(v.y); }
-            Vec2<TY>::st(y + off, v);
-        }
-    }
-}
-
-// ---- large tensors (VAE 512^2 / 256^2 maps: too big for the fused kernel's shared memory): the same two passes, but the
-// rows stream through a 3-stage ring of 32 KiB cp.async.bulk (TMA 1-D) chunks, so every CTA keeps ~64-96 KiB in flight
-// instead of a few 8-byte loads per thread.
+// ---- GroupNorm forward for tensors whose rows do not fit the cluster kernel's shared memory (VAE 512^2 / 256^2 maps, large
+// batches): a statistics pass and an apply pass, with the rows streaming through a 3-stage ring of 32 KiB
+// cp.async.bulk (TMA 1-D) chunks, so every CTA keeps ~64-96 KiB in flight instead of a few 8-byte loads per thread.
 constexpr int kGnTmaStages = 3;
 constexpr int kGnTmaChunkBytes = 32768;
 
@@ -474,280 +387,13 @@ gn_bwd_apply_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const f
     }
 }
 
-// ---- single-kernel GroupNorm for tensors that fit in the SMs' shared memory (every UNet activation at bs=1) -----
-// grid = (row blocks, images) with at most one CTA per SM, so all CTAs are co-resident: each CTA loads its rows ONCE
-// into shared memory while accumulating the group sums, publishes them with fp64 atomics, waits on a grid-wide
-// arrival counter, then normalises straight out of shared memory.  x is read from HBM/L2 once instead of twice and
-// the statistics + apply passes are one launch.
-// counter[0] = arrivals, counter[1] = departures.  Arrival is a fire-and-forget red.add and the wait is a plain poll,
-// so the critical path after the last arrival is one L2 round trip.  Every CTA also counts its departure; the last one
-// to leave (off the critical path) clears both words, so the pair is reusable by the next call without a memset node
-// (the workspace is zeroed once by its owner).  Requires all CTAs of the grid to be co-resident.
-__device__ __forceinline__ void grid_arrive_and_wait(unsigned* counter, unsigned expected) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-        unsigned seen;
-        do {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-        } while (seen < expected);
-    }
-    __syncthreads();
-}
-__device__ __forceinline__ void grid_depart(unsigned* counter, unsigned expected) {
-    if (threadIdx.x == 0) {
-        if (atomicAdd(counter + 1, 1u) == expected - 1) {
-            counter[0] = 0;
-            counter[1] = 0;
-        }
-    }
-}
-
-// Cross-CTA reduction without same-address atomics (which serialise in L2): every CTA publishes its per-group partial
-// sums to its own slot part[(n*nb + block)*G + g]; after the grid barrier each CTA folds the nb partials of its image
-// (kFoldSlices x G threads, each with a handful of independent L2 loads in flight, then one pass over shared memory).
-constexpr int kFoldSlices = 16;
-__device__ __forceinline__ void publish_partials(float2* __restrict__ part, const float* s_a, const float* s_b, int G) {
-    if (threadIdx.x < G)
-        part[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * G + threadIdx.x] = make_float2(s_a[threadIdx.x], s_b[threadIdx.x]);
-}
-__device__ __forceinline__ void fold_partials(const float2* __restrict__ part, double2 (*s_fold)[64], double* s_d0,
-                                              double* s_d1, int G) {
-    const int g = threadIdx.x % G, slice = threadIdx.x / G;
-    const int nslices = min(kFoldSlices, (int)blockDim.x / G);
-    const int nb = gridDim.x;
-    if (slice < nslices) {
-        double a = 0.0, b = 0.0;
-        const float2* pp = part + (size_t)blockIdx.y * nb * G + g;
-        for (int blk = slice; blk < nb; blk += 4 * nslices) {
-            float2 v[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int bi = blk + u * nslices;
-                v[u] = bi < nb ? __ldcg(pp + (size_t)bi * G) : make_float2(0.f, 0.f);
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) { a += v[u].x; b += v[u].y; }
-        }
-        s_fold[slice][g] = make_double2(a, b);
-    }
-    __syncthreads();
-    if (threadIdx.x < G) {
-        double a = 0.0, b = 0.0;
-        for (int i = 0; i < nslices; ++i) { a += s_fold[i][threadIdx.x].x; b += s_fold[i][threadIdx.x].y; }
-        s_d0[threadIdx.x] = a;
-        s_d1[threadIdx.x] = b;
-    }
-    __syncthreads();
-}
-
-// The CTA's rows are one contiguous range of the [HW][C] matrix: a single cp.async.bulk (TMA, 1-D) stages them in
-// shared memory -- the whole range is in flight at once instead of two 8-byte loads per thread.
-template <typename TX, typename TY>
-__global__ void __launch_bounds__(kGnFusedThreads)
-gn_fused_fwd_kernel(const TX* __restrict__ x, TY* __restrict__ y, const float* __restrict__ gamma,
-                    const float* __restrict__ beta, double* __restrict__ ws, unsigned* __restrict__ counter,
-                    float* __restrict__ mean_out, float* __restrict__ rstd_out, int HW, int C, int G, float eps, int act,
-                    int rows_per_block, int PW, int RY, int chunks) {
-    extern __shared__ __align__(128) unsigned char gn_smem[];
-    TX* sx = reinterpret_cast<TX*>(gn_smem);
-    __shared__ float s_a[64], s_b[64];
-    __shared__ double s_d0[64], s_d1[64];
-    __shared__ double2 s_fold[kFoldSlices][64];
-    __shared__ __align__(8) unsigned long long s_bar;
-    const int n = blockIdx.y;
-    const int tx = threadIdx.x % PW, ty = threadIdx.x / PW;
-    const int r0 = blockIdx.x * rows_per_block;
-    const int r1 = min(HW, r0 + rows_per_block);
-    const int cpg = C / G;
-    const uint32_t bar = smem_u32(&s_bar);
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    if (threadIdx.x < 64) { s_a[threadIdx.x] = 0.f; s_b[threadIdx.x] = 0.f; }
-    group_acc_begin();
-    __syncthreads();
-    pdl_sync();
-    if (threadIdx.x == 0 && r1 > r0) {
-        const uint32_t bytes = (uint32_t)((size_t)(r1 - r0) * C * sizeof(TX));
-        mbar_arrive_expect_tx(bar, bytes);
-        tma_bulk_g2s(smem_u32(sx), x + ((size_t)n * HW + r0) * C, bytes, bar);
-    }
-    if (r1 > r0) mbar_wait(bar, 0);
-    float a1[kGnMaxChunks], a2[kGnMaxChunks];
-#pragma unroll
-    for (int j = 0; j < kGnMaxChunks; ++j) { a1[j] = 0.f; a2[j] = 0.f; }
-#pragma unroll 4
-    for (int r = r0 + ty; r < r1; r += RY) {
-        const TX* sr = sx + (size_t)(r - r0) * C + 2 * tx;
-#pragma unroll
-        for (int j = 0; j < kGnMaxChunks; ++j) {
-            if (j < chunks) {
-                const float2 v = Vec2<TX>::ld(sr + 2 * j * PW);
-                a1[j] += v.x + v.y;
-                a2[j] += v.x * v.x + v.y * v.y;
-            }
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < kGnMaxChunks; ++j) {
-        if (j < chunks) {
-            const int g = (2 * (tx + j * PW)) / cpg;
-            group_accumulate(s_a, s_b, g, a1[j], a2[j]);
-        }
-    }
-    __syncthreads();
-    group_acc_flush(s_a, s_b, 64);
-    float2* part = reinterpret_cast<float2*>(ws);
-    publish_partials(part, s_a, s_b, G);
-    grid_arrive_and_wait(counter, gridDim.x * gridDim.y);
-    fold_partials(part, s_fold, s_d0, s_d1, G);
-    grid_depart(counter, gridDim.x * gridDim.y);
-    if (threadIdx.x < G) {
-        const double cnt = (double)HW * cpg;
-        const double m = s_d0[threadIdx.x] / cnt;
-        double var = s_d1[threadIdx.x] / cnt - m * m;
-        if (var < 0) var = 0;
-        const float rs = (float)(1.0 / sqrt(var + (double)eps));
-        s_a[threadIdx.x] = (float)m;
-        s_b[threadIdx.x] = rs;
-        if (blockIdx.x == 0) {
-            mean_out[n * G + threadIdx.x] = (float)m;
-            rstd_out[n * G + threadIdx.x] = rs;
-        }
-    }
-    __syncthreads();
-    const size_t base = ((size_t)n * HW) * C;
-    for (int j = 0; j < chunks; ++j) {
-        const int c = 2 * (tx + j * PW);
-        const int g = c / cpg;
-        const float m = s_a[g], rs = s_b[g];
-        const float g0 = gamma[c] * rs, g1 = gamma[c + 1] * rs;
-        const float b0 = beta[c] - m * g0, b1 = beta[c + 1] - m * g1;
-#pragma unroll 4
-        for (int r = r0 + ty; r < r1; r += RY) {
-            float2 v = Vec2<TX>::ld(sx + (size_t)(r - r0) * C + c);
-            v.x = v.x * g0 + b0;
-            v.y = v.y * g1 + b1;
-            if (act) { v.x = silu_f(v.x); v.y = silu_f(v.y); }
-            Vec2<TY>::st(y + base + (size_t)r * C + c, v);
-        }
-    }
-}
-
-template <typename TX, typename TG, typename TD>
-__global__ void __launch_bounds__(kGnFusedThreads)
-gn_fused_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const float* __restrict__ gamma,
-                    const float* __restrict__ beta, const float* __restrict__ mean, const float* __restrict__ rstd,
-                    double* __restrict__ ws, unsigned* __restrict__ counter, TD* __restrict__ dx, TG* __restrict__ dx_lp,
-                    int HW, int C, int G, int act, int accumulate, int rows_per_block, int PW, int RY, int chunks) {
-    // shared memory stages this CTA's rows of x and dy (two bulk copies); xhat / dz*gamma are recomputed from them
-    extern __shared__ __align__(128) unsigned char gn_smem[];
-    TX* sx = reinterpret_cast<TX*>(gn_smem);
-    TG* sdy = reinterpret_cast<TG*>(gn_smem + (((size_t)rows_per_block * C * sizeof(TX) + 127) & ~(size_t)127));
-    __shared__ float s_1[64], s_2[64];
-    __shared__ double s_d0[64], s_d1[64];
-    __shared__ double2 s_fold[kFoldSlices][64];
-    __shared__ __align__(8) unsigned long long s_bar;
-    const int n = blockIdx.y;
-    const int tx = threadIdx.x % PW, ty = threadIdx.x / PW;
-    const int cpg = C / G;
-    const int r0 = blockIdx.x * rows_per_block;
-    const int r1 = min(HW, r0 + rows_per_block);
-    const uint32_t bar = smem_u32(&s_bar);
-    if (threadIdx.x == 0) {
-        mbar_init(bar, 1);
-        mbar_fence_init();
-        fence_proxy_async_smem();
-    }
-    if (threadIdx.x < 64) { s_1[threadIdx.x] = 0.f; s_2[threadIdx.x] = 0.f; }
-    group_acc_begin();
-    __syncthreads();
-    pdl_sync();
-    const size_t base = ((size_t)n * HW) * C;
-    if (threadIdx.x == 0 && r1 > r0) {
-        const uint32_t bx = (uint32_t)((size_t)(r1 - r0) * C * sizeof(TX)), bd = (uint32_t)((size_t)(r1 - r0) * C * sizeof(TG));
-        mbar_arrive_expect_tx(bar, bx + bd);
-        tma_bulk_g2s(smem_u32(sx), x + base + (size_t)r0 * C, bx, bar);
-        tma_bulk_g2s(smem_u32(sdy), dy + base + (size_t)r0 * C, bd, bar);
-    }
-    if (r1 > r0) mbar_wait(bar, 0);
-    for (int j = 0; j < chunks; ++j) {
-        const int c = 2 * (tx + j * PW);
-        const int g = c / cpg;
-        const float m = mean[n * G + g], rs = rstd[n * G + g];
-        const float ga0 = gamma[c], ga1 = gamma[c + 1], be0 = beta[c], be1 = beta[c + 1];
-        float a1 = 0.f, a2 = 0.f;
-#pragma unroll 4
-        for (int r = r0 + ty; r < r1; r += RY) {
-            const size_t so = (size_t)(r - r0) * C + c;
-            const float2 xv = Vec2<TX>::ld(sx + so);
-            float2 d = Vec2<TG>::ld(sdy + so);
-            const float xh0 = (xv.x - m) * rs, xh1 = (xv.y - m) * rs;
-            if (act) {
-                d.x *= silu_grad(xh0 * ga0 + be0);
-                d.y *= silu_grad(xh1 * ga1 + be1);
-            }
-            const float t0 = d.x * ga0, t1 = d.y * ga1;
-            a1 += t0 + t1;
-            a2 += t0 * xh0 + t1 * xh1;
-        }
-        group_accumulate(s_1, s_2, g, a1, a2);
-    }
-    __syncthreads();
-    group_acc_flush(s_1, s_2, 64);
-    float2* part = reinterpret_cast<float2*>(ws);
-    publish_partials(part, s_1, s_2, G);
-    grid_arrive_and_wait(counter, gridDim.x * gridDim.y);
-    fold_partials(part, s_fold, s_d0, s_d1, G);
-    grid_depart(counter, gridDim.x * gridDim.y);
-    if (threadIdx.x < G) {
-        const double cnt = (double)HW * cpg;
-        s_1[threadIdx.x] = (float)(s_d0[threadIdx.x] / cnt);
-        s_2[threadIdx.x] = (float)(s_d1[threadIdx.x] / cnt);
-    }
-    __syncthreads();
-    for (int j = 0; j < chunks; ++j) {
-        const int c = 2 * (tx + j * PW);
-        const int g = c / cpg;
-        const float m = mean[n * G + g], rs = rstd[n * G + g];
-        const float ga0 = gamma[c], ga1 = gamma[c + 1], be0 = beta[c], be1 = beta[c + 1];
-        const float m1 = s_1[g], m2 = s_2[g];
-#pragma unroll 4
-        for (int r = r0 + ty; r < r1; r += RY) {
-            const size_t so = (size_t)(r - r0) * C + c;
-            const float2 xv = Vec2<TX>::ld(sx + so);
-            float2 d = Vec2<TG>::ld(sdy + so);
-            const float xh0 = (xv.x - m) * rs, xh1 = (xv.y - m) * rs;
-            if (act) {
-                d.x *= silu_grad(xh0 * ga0 + be0);
-                d.y *= silu_grad(xh1 * ga1 + be1);
-            }
-            float2 o;
-            o.x = rs * (d.x * ga0 - m1 - xh0 * m2);
-            o.y = rs * (d.y * ga1 - m1 - xh1 * m2);
-            const size_t off = base + (size_t)r * C + c;
-            if (accumulate) {
-                const float2 p = Vec2<TD>::ld(dx + off);
-                o.x += p.x;
-                o.y += p.y;
-            }
-            Vec2<TD>::st(dx + off, o);
-            if (dx_lp) Vec2<TG>::st(dx_lp + off, o);      // 16-bit copy for the dgrad GEMM that consumes dx next
-        }
-    }
-}
-
-// ---- GroupNorm on thread-block clusters: no grid-wide barrier ----------------------------------------------------------
+// ---- GroupNorm on thread-block clusters: one launch, x read once ------------------------------------------------------
 // A cluster owns a SLAB of `gpc` consecutive groups (cw = gpc * C/G channels) of one image for ALL rows; its S CTAs split
 // the rows.  Every CTA stages its rows x cw sub-matrix in shared memory (read once), the per-group partial sums of the S
 // CTAs meet through distributed shared memory (each CTA stores its gpc (sum, sumsq) pairs into every peer: S*gpc 8-byte
-// remote stores, one cluster barrier), and the normalised rows are written straight from shared memory.  Compared with the
-// single-kernel variant above there is no arrival counter to spin on, no 147-way fold of partial sets out of L2, and no
-// requirement that all CTAs of the grid be resident at once (util.py:199-216 GroupNorm32, openaimodel.py:201-241).
+// remote stores, one cluster barrier), and the normalised rows are written straight from shared memory.  CTAs wait only on
+// the peers of their own cluster, which the hardware co-schedules, so the grid needs no global barrier and need not be
+// resident at once (util.py:199-216 GroupNorm32, openaimodel.py:201-241).
 constexpr int kGnClThreads = 512;
 constexpr int kGnClMaxS = 16;
 
@@ -983,12 +629,11 @@ gn_cluster_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const
 }
 
 // cluster shape for (N images, HW rows, C channels, G groups): slabs of gpc groups, S CTAs per slab.  Returns false when
-// the staged rows do not fit in shared memory (the streaming / single-kernel variants take over).
-static bool g_gn_cluster_unavailable = false;     // set when a cluster launch was refused: the other variants take over
+// the staged rows do not fit in shared memory (the statistics + apply kernel pairs take over).
+static bool g_gn_cluster_unavailable = false;     // set when a cluster launch was refused: the kernel pairs take over
 struct GnClPlan { int S, gpc, rows_per_cta; size_t smem; };
 static inline bool gn_cluster_plan(int N, int HW, int C, int G, size_t bytes_per_elem, GnClPlan* out) {
-    static const int on = getenv("CB_GN_CLUSTER") ? atoi(getenv("CB_GN_CLUSTER")) : 1;
-    if (!on || G > 32) return false;
+    if (G > 32) return false;
     const int cpg = C / G;
     const int sms = device_sm_count();
     for (int gpc : {4, 8, 2, 16, 1, 32}) {
@@ -1115,7 +760,8 @@ ln_bwd_kernel(const TG* __restrict__ dy, const TX* __restrict__ x, const float* 
     }
 }
 
-// CTAs per image whose (sum, sumsq) partials (float2 per group) fit the caller's workspace
+// CTAs per image whose (sum, sumsq) partials (float2 per group) fit the caller's workspace.  The last 8 bytes stay out of
+// the budget: the partials are added in CTA order, so a different CTA count would change the results' bits.
 static inline int gn_max_blocks(int N, int G) { return std::max(1, (int)((CB_GN_WS_BYTES - 8) / (8 * (size_t)G * N))); }
 static inline int gn_rows_per_block(int HW, int N, int G) {
     const int target_blocks = 8 * device_sm_count();     // 256-thread blocks: 8 per SM keep 2048 threads x 8 loads in flight
@@ -1158,21 +804,18 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
                                 double* ws, void* stream) {
     int rc = gn_check(N, HW, C, G);
     if (rc) return rc;
+    // the streaming pair stages whole rows with cp.async.bulk, whose sizes and addresses are multiples of 16 bytes;
+    // checked here, before any launch, so that a shape is accepted or refused the same way on every device
+    const size_t row_bytes = (size_t)C * (x_dtype == CB_F32 ? 4 : 2);
+    CB_REQUIRE(row_bytes % 16 == 0, CB_ERR_ARG, "groupnorm_fwd: rows must be multiples of 16 bytes (C=%d, x dtype %d)", C,
+               x_dtype);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    // flags: bit 0 = fuse SiLU, bit 1 = CB_GN_NO_GRID_BARRIER (never launch the single-kernel variant whose CTAs spin on a
-    // grid-wide arrival counter: required on any stream that runs concurrently with another GroupNorm stream)
-    const bool allow_fused = (act_silu & CB_GN_NO_GRID_BARRIER) == 0;
-    // bits 8..23: upper bound on the CTAs of the streaming two-kernel path (0 = two per SM): a front end that shares the
-    // device with a latency-bound chain of small launches leaves the other SMs to it
+    // flags: bit 0 = fuse SiLU; bits 8..23: upper bound on the CTAs of the streaming two-kernel path (0 = two per SM): a
+    // front end that shares the device with a latency-bound chain of small launches leaves the other SMs to it
     const int cta_cap = (act_silu >> 8) & 0xFFFF;
     act_silu &= 1;
-    // ws: CB_GN_WS_BYTES; [0, 2*N*G doubles) group sums of the two-kernel path, or per-CTA partial slots of the fused
-    // path; the last 8 bytes hold the grid arrival counter
-    unsigned* counter = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(ws) + CB_GN_WS_BYTES - 8);
-    const GnShape gs = gn_shape(C);
-    const int nthr = gs.pw * gs.ry;
     {
-        // cluster path: slabs of groups, statistics through distributed shared memory (no grid-wide barrier)
+        // cluster path: slabs of groups, statistics through distributed shared memory
         GnClPlan pl;
         if (!g_gn_cluster_unavailable && gn_cluster_plan(N, HW, C, G, x_dtype == CB_F32 ? 4 : 2, &pl)) {
             dim3 gridc((unsigned)pl.S, (unsigned)(G / pl.gpc), (unsigned)N);
@@ -1196,68 +839,33 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
                 return 0;
             }
             // this device cannot co-schedule the cluster (or refuses the attributes): clear the launch error and use the
-            // single-kernel / streaming variants from now on
+            // streaming pair from now on
             (void)cudaGetLastError();
             g_gn_cluster_unavailable = true;
         }
     }
-    {
-        // fused single-kernel path: all CTAs co-resident (<= 1 per SM) and each CTA's rows fit in shared memory
-        const int sms = device_sm_count();
-        const int nb = sms / N;
-        const int xes = x_dtype == CB_F32 ? 4 : 2;
-        if (nb >= 1 && allow_fused) {
-            const int rpbf = ceil_div(HW, nb);
-            const size_t smem = (size_t)rpbf * C * xes;
-            if (smem <= kGnMaxDynSmem && ((size_t)C * xes) % 16 == 0) {
-                dim3 gridf(ceil_div(HW, rpbf), N);
-                CB_REQUIRE((size_t)gridf.x * N * G * 8 <= CB_GN_WS_BYTES - 8, CB_ERR_ARG, "groupnorm: workspace too small");
-                const int ryf = std::max(1, std::min(rpbf, kGnFusedThreads / gs.pw));
-                CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY, {
-                    auto kern = gn_fused_fwd_kernel<TX, TY>;
-                    static size_t max_set = 0;
-                    if (smem > max_set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem)); max_set = kGnMaxDynSmem; }
-                    CB_LAUNCH((kern), gridf, gs.pw * ryf, smem, st, (const TX*)x, (TY*)y, gamma, beta, ws, counter, mean_out, rstd_out, HW, C, G, eps, act_silu, rpbf, gs.pw, ryf, gs.chunks);
-                }));
-                CB_CUDA(cudaGetLastError());
-                cb::count_launches(1);
-                return 0;
-            }
-        }
-    }
-    {
-        // streaming (TMA-staged) variant: rows are 16-byte multiples and a chunk of them fits one 32 KiB stage
-        const int xes = x_dtype == CB_F32 ? 4 : 2;
-        const size_t row_bytes = (size_t)C * xes;
-        const int rpc = (int)(kGnTmaChunkBytes / row_bytes);
-        if (row_bytes % 16 == 0 && rpc >= 1) {
-            const int ctas = cta_cap > 0 ? std::min(cta_cap, 2 * device_sm_count()) : 2 * device_sm_count();
-            const int nb = std::max(1, std::min(ctas / N, gn_max_blocks(N, G)));
-            const int rpbt = ceil_div(HW, nb);
-            dim3 gridt(ceil_div(HW, rpbt), N);
-            const size_t smem = (size_t)kGnTmaStages * kGnTmaChunkBytes;
-            CB_DISPATCH_2(x_dtype, TX, {
-                auto kern = gn_stats_tma_kernel<TX>;
-                static bool set = false;
-                if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set = true; }
-                CB_LAUNCH((kern), gridt, nthr, smem, st, (const TX*)x, ws, HW, C, G, rpbt, rpc, gs.pw, gs.ry, gs.chunks);
-            });
-            CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY, {
-                auto kern = gn_apply_tma_kernel<TX, TY>;
-                static bool set = false;
-                if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set = true; }
-                CB_LAUNCH((kern), gridt, nthr, smem, st, (const TX*)x, (TY*)y, gamma, beta, ws, mean_out, rstd_out, HW, C, G, eps, act_silu, rpbt, rpc, gs.pw, gs.ry, gs.chunks);
-            }));
-            CB_CUDA(cudaGetLastError());
-            cb::count_launches(2);
-            return 0;
-        }
-    }
-    const int rpb = gn_rows_per_block(HW, N, G);
-    dim3 grid(ceil_div(HW, rpb), N);
-    CB_DISPATCH_2(x_dtype, TX,CB_LAUNCH((gn_stats_kernel<TX>), grid, nthr, 0, st, (const TX*)x, ws, HW, C, G, rpb, gs.pw, gs.ry, gs.chunks));
-    CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY,
-CB_LAUNCH((gn_apply_kernel<TX, TY>), grid, nthr, 0, st, (const TX*)x, (TY*)y, gamma, beta, ws, mean_out, rstd_out, HW, C, G, eps, act_silu, rpb, gs.pw, gs.ry, gs.chunks)));
+    // streaming (TMA-staged) pair.  ws: one (sum, sumsq) float2 partial per (image, CTA, group), added up in CTA order.
+    // gn_check bounds C to 4096, so a row is at most 16 KiB and a 32 KiB stage holds at least two.
+    const GnShape gs = gn_shape(C);
+    const int nthr = gs.pw * gs.ry;
+    const int rpc = (int)(kGnTmaChunkBytes / row_bytes);
+    const int ctas = cta_cap > 0 ? std::min(cta_cap, 2 * device_sm_count()) : 2 * device_sm_count();
+    const int nb = std::max(1, std::min(ctas / N, gn_max_blocks(N, G)));
+    const int rpbt = ceil_div(HW, nb);
+    dim3 gridt(ceil_div(HW, rpbt), N);
+    const size_t smem = (size_t)kGnTmaStages * kGnTmaChunkBytes;
+    CB_DISPATCH_2(x_dtype, TX, {
+        auto kern = gn_stats_tma_kernel<TX>;
+        static bool set = false;
+        if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set = true; }
+        CB_LAUNCH((kern), gridt, nthr, smem, st, (const TX*)x, ws, HW, C, G, rpbt, rpc, gs.pw, gs.ry, gs.chunks);
+    });
+    CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(y_dtype, TY, {
+        auto kern = gn_apply_tma_kernel<TX, TY>;
+        static bool set = false;
+        if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); set = true; }
+        CB_LAUNCH((kern), gridt, nthr, smem, st, (const TX*)x, (TY*)y, gamma, beta, ws, mean_out, rstd_out, HW, C, G, eps, act_silu, rpbt, rpc, gs.pw, gs.ry, gs.chunks);
+    }));
     CB_CUDA(cudaGetLastError());
     cb::count_launches(2);
     return 0;
@@ -1270,11 +878,9 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
     int rc = gn_check(N, HW, C, G);
     if (rc) return rc;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    unsigned* counter = reinterpret_cast<unsigned*>(reinterpret_cast<char*>(ws) + CB_GN_WS_BYTES - 8);
     const GnShape gs = gn_shape(C);
     const int nthr = gs.pw * gs.ry;
     CB_REQUIRE(dx_dtype == CB_F32 || dx_dtype == dy_dtype, CB_ERR_ARG, "groupnorm_bwd: dx dtype must be f32 or equal dy dtype");
-    const bool allow_fused = (act_silu & CB_GN_NO_GRID_BARRIER) == 0;
     act_silu &= 1;
     {
         GnClPlan pl;
@@ -1307,32 +913,7 @@ extern "C" int cb_groupnorm_bwd(const void* dy, int dy_dtype, const void* x, int
             g_gn_cluster_unavailable = true;
         }
     }
-    {
-        const int sms = device_sm_count();
-        const int nb = sms / N;
-        if (nb >= 1 && allow_fused) {
-            const int rpbf = ceil_div(HW, nb);
-            const int xes = x_dtype == CB_F32 ? 4 : 2, ges = dy_dtype == CB_F32 ? 4 : 2;
-            const size_t smem = (((size_t)rpbf * C * xes + 127) & ~(size_t)127) + (size_t)rpbf * C * ges;   // staged x + dy
-            if (smem <= kGnMaxDynSmem && ((size_t)C * xes) % 16 == 0 && ((size_t)C * ges) % 16 == 0) {
-                dim3 gridf(ceil_div(HW, rpbf), N);
-                CB_REQUIRE((size_t)gridf.x * N * G * 8 <= CB_GN_WS_BYTES - 8, CB_ERR_ARG, "groupnorm: workspace too small");
-                const int ryf = std::max(1, std::min(rpbf, kGnFusedThreads / gs.pw));
-#define CB_GN_BWD_FUSED(TDX)                                                                                                      \
-                CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(dy_dtype, TG, {                                                              \
-                    auto kern = gn_fused_bwd_kernel<TX, TG, TDX>;                                                                     \
-                    static bool set = false;                                                                                         \
-                    if (!set) { CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kGnMaxDynSmem)); set = true; } \
-                    CB_LAUNCH((kern), gridf, gs.pw * ryf, smem, st, (const TG*)dy, (const TX*)x, gamma, beta, mean, rstd, ws, counter, (TDX*)dx, (TG*)dx_lp, HW, C, G, act_silu, accumulate, rpbf, gs.pw, ryf, gs.chunks); \
-                }))
-                if (dx_dtype == CB_F32) { CB_GN_BWD_FUSED(float); } else { CB_GN_BWD_FUSED(TG); }
-#undef CB_GN_BWD_FUSED
-                CB_CUDA(cudaGetLastError());
-                cb::count_launches(1);
-                return 0;
-            }
-        }
-    }
+    // statistics + apply pair.  ws: one (sum, sumsq) float2 partial per (image, CTA, group), added up in CTA order
     const int rpb = gn_rows_per_block(HW, N, G);
     dim3 grid(ceil_div(HW, rpb), N);
     CB_DISPATCH_2(x_dtype, TX, CB_DISPATCH_2(dy_dtype, TG,

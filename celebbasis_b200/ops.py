@@ -72,9 +72,8 @@ def _splitk_workspace(device):
 # later launches -- including the ones captured into the step graph -- pass the winner in desc.tile_n / desc.splits.
 AUTOTUNE = os.environ.get("CB_GEMM_AUTOTUNE", "1") != "0"
 # split-K slices as a thread-block cluster reducing through DSMEM (desc.splitk_cluster): an autotuner candidate on the lane-0
-# stream (=1, default), on every lane (=2) or never (=0).  Lane 0 is the default because a GroupNorm that falls back to the
-# single-kernel variant (CTAs spinning on a grid-wide counter) is then ordered with the cluster GEMMs by the stream; a pending
-# cluster and a half-resident spinning grid on concurrent streams could wait for each other.
+# stream (=1, default), on every lane (=2) or never (=0).  Lane 0 is the default because the lanes other than 0 were tuned
+# and measured without cluster split-K; whether it helps beside concurrent streams has not been measured.
 CLUSTER_SK = os.environ.get("CB_GEMM_CLUSTER_SK", "1") != "0"
 CLUSTER_SK_ALL_LANES = os.environ.get("CB_GEMM_CLUSTER_SK", "1") == "2"   # A/B aid: also beside concurrent streams
 # Front-end SM budget (CB_FE_CTAS = n > 0): the software-pipelined front end (VAE encode of the NEXT batch, lane 2) runs
@@ -227,10 +226,8 @@ def _gemm(d, what):
         if win is None and not torch.cuda.is_current_stream_capturing():
             win = _autotune(d, key)
         if win is not None:
-            # Cluster split-K only on the lane-0 stream: a cluster of 6..16 CTAs must be co-scheduled inside one GPC, and the
-            # single-kernel GroupNorm (lane 0 only) spins on a grid-wide arrival counter until all its CTAs are resident.  On
-            # one stream the two are ordered; on concurrent streams a pending cluster at the head of the block scheduler's
-            # queue and a half-resident spinning grid can wait for each other forever (observed: the step hangs).
+            # Cluster split-K only on the lane-0 stream (see CLUSTER_SK): the other lanes keep the configuration they were
+            # tuned and measured with, the best one without cluster split-K.
             if win[4] == 1 and _LANE != 0 and not CLUSTER_SK_ALL_LANES:
                 win = _TUNE_NC.get(key, (0, 0, 0, 0, 0))
             d.tile_n, d.splits, d.stages, d.cta_pair, d.splitk_cluster = win
@@ -449,15 +446,10 @@ def _gn_ws(device, n):
     return ws
 
 
-GN_NO_GRID_BARRIER = False    # set (or run under lane != 0) to force the barrier-free statistics + apply kernel pair
-
-
 def _gn_flags(silu):
-    """bit 0: fused SiLU; bit 1 (CB_GN_NO_GRID_BARRIER): the single-kernel GroupNorm spins on a grid-wide arrival counter
-    and needs all its CTAs co-resident -- only the lane-0 stream may use it (two such kernels on concurrent streams could
-    each hold part of the SMs and wait for the rest forever)."""
+    """bit 0: fused SiLU; bits 8..23 (CB_GN_CTA_CAP(n)): the front-end SM budget of the streaming GroupNorm pair."""
     cap = (FE_CTAS & 0xFFFF) << 8 if (FE_CTAS > 0 and _LANE in FE_LANES) else 0     # CB_GN_CTA_CAP(n)
-    return (1 if silu else 0) | (2 if (_LANE != 0 or GN_NO_GRID_BARRIER) else 0) | cap
+    return (1 if silu else 0) | cap
 
 
 def groupnorm(x, geo, gamma, beta, *, groups=32, eps=1e-5, silu=False, out_dtype=torch.float16, want_stats=True):

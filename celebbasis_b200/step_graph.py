@@ -14,8 +14,8 @@ Three graphs over static buffers (torch is buffers / streams / graph capture onl
   G_pipe  promote next->cur; chain on (z_cur, v_cur)  ||  front end of the new `next` batch  (steady state)
 
 The chain runs on a high-priority stream (its many small kernels should never queue behind a wave of VAE CTAs); the
-front end runs with ops.lane(1/2) workspaces and barrier-free GroupNorm kernels, so the chain's single-kernel GroupNorm
-(grid-wide arrival counter) never shares the device with another spinning kernel.
+front end runs with ops.lane(1/2) workspaces, so its split-K and GroupNorm launches never share a workspace with the
+chain's concurrent ones.
 """
 import torch
 

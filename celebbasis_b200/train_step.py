@@ -196,8 +196,8 @@ class CelebBasisStep:
         T = ids_dev.shape[1]
         # Two independent branches until the UNet: (a) face net -> celeb-basis MLP -> CLIP text (small, latency-bound
         # launches that use few SMs) and (b) VAE encode + q_sample (large, throughput-bound convs).  They run on two
-        # streams (fork/join with events; a captured graph keeps them as parallel branches).  Branch (a) never launches
-        # a grid-barrier kernel (no GroupNorm), so the fused GroupNorm of branch (b) keeps its co-residency guarantee.
+        # streams (fork/join with events; a captured graph keeps them as parallel branches), each with its own
+        # workspace lane.
         main = torch.cuda.current_stream()
         overlap = self.overlap_branches and self._warm      # first call: sequential, so the GEMM autotuner times alone
         self._warm = True
@@ -259,7 +259,7 @@ class CelebBasisStep:
     # ------------------------------------------------------------------------------------------
     def stage_prefetch(self, image, faces, n_chunks, posterior_eps, z_out=None, v_out=None):
         """get_input's VAE encode + posterior sample (ddpm.py:702-759) and the CosFace features of the face crops
-        (meta_net.py:329-346, no_grad): two concurrent branches, neither uses a grid-barrier kernel (lanes 1 / 2)."""
+        (meta_net.py:329-346, no_grad): two concurrent branches with their own workspaces (lanes 1 / 2)."""
         main = torch.cuda.current_stream()
         side = self._side_stream()
         fork = torch.cuda.Event()

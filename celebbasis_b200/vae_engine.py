@@ -3,8 +3,8 @@
 Mirrors ldm/models/autoencoder.py:324-328 -> ldm/modules/diffusionmodules/model.py:434-459 (Encoder.forward),
 :82-141 (ResnetBlock), :150-202 (AttnBlock: 1 head over all pixels), :60-79 (Downsample: pad (0,1,0,1) + stride 2).
 The largest single item of a training step (1.1 TFLOP at 512x512): every conv is the same TMA-shifted implicit
-GEMM as the UNet's, GroupNorm(eps 1e-6)+swish is the fused norm kernel, the 4096-token attention reuses the
-batched GEMM + softmax path with head_dim = 512.
+GEMM as the UNet's, GroupNorm(eps 1e-6)+swish is one cb_groupnorm_fwd call with the SiLU fused, the 4096-token
+attention reuses the batched GEMM + softmax path with head_dim = 512.
 """
 import torch
 

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define CB_ABI_VERSION 5
+#define CB_ABI_VERSION 6
 #define CB_GN_WS_BYTES 131072
 
 /* element types */
@@ -180,8 +180,7 @@ int cb_gemm(const cb_gemm_desc* desc, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Normalisation (channels-last).  ws = caller workspace of CB_GN_WS_BYTES bytes (per-CTA partial sums, added up in
- * CTA order, plus a self-resetting grid arrival counter in its last 8 bytes); the caller zeroes it ONCE at allocation;
- * calls sharing it must be stream-ordered.
+ * CTA order); it needs no initialisation, and calls sharing it must be stream-ordered.
  * cb_groupnorm_*: ldm/modules/diffusionmodules/util.py:199-216 (GroupNorm32, eps 1e-5),
  *   ldm/modules/attention.py:76-77 and ldm/modules/diffusionmodules/model.py:38-39 (Normalize, eps 1e-6),
  *   optionally fused with the nn.SiLU that follows (openaimodel.py:201-241, model.py:33-35 nonlinearity).
@@ -189,14 +188,16 @@ int cb_gemm(const cb_gemm_desc* desc, void* stream);
  * The *_bwd entry points are the activation gradients torch.autograd computes in the reference
  * (SURVEY.md §8 a29); accumulate != 0 adds into dx (residual-branch join).
  * ------------------------------------------------------------------------------------------- */
-/* cb_groupnorm_bwd: dx_lp (optional, dtype of dy): the result is also written as a 16-bit copy -- the operand of the
- * dgrad GEMM that consumes dx next (saves a cast launch per ResBlock / transformer block of the backward pass). */
-#define CB_GN_NO_GRID_BARRIER 2 /* OR into act_silu: force the statistics + apply kernel pair (no grid-wide spin barrier) */
+/* cb_groupnorm_fwd: rows of x must be multiples of 16 bytes (C * sizeof(x) % 16 == 0; CB_ERR_ARG otherwise).
+ * cb_groupnorm_bwd: dx_lp (optional, dtype of dy): the result is also written as a 16-bit copy -- the operand of the
+ * dgrad GEMM that consumes dx next (saves a cast launch per ResBlock / transformer block of the backward pass).
+ * act_silu: bit 0 = fuse SiLU; bits 8..23 = CB_GN_CTA_CAP(n); other bits are ignored. */
 #define CB_GN_CTA_CAP(n) (((n) & 0xFFFF) << 8) /* OR into act_silu (cb_groupnorm_fwd): at most n CTAs on the streaming kernel pair */
 /* How cb_groupnorm_fwd / _bwd would run a (N, HW, C, G) problem whose staged element costs `bytes_per_elem` bytes
  * (fwd: sizeof(x); bwd: sizeof(x) + sizeof(dy)): returns 1 and fills plan[4] = {CTAs per cluster, groups per cluster slab,
  * rows per CTA, dynamic shared memory bytes} when the thread-block-cluster variant applies (slabs of groups, statistics
- * through distributed shared memory), 0 when the rows do not fit and the single-kernel / streaming variants take over.
+ * through distributed shared memory), 0 when the rows do not fit and a statistics + apply kernel pair takes over
+ * (forward: rows streamed through shared memory by TMA; backward: plain loads).
  * Host-only (no launch): lets integrators and the CPU tests see the launch geometry. */
 int cb_groupnorm_cluster_plan(int N, int HW, int C, int G, int bytes_per_elem, int* plan);
 int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype, const float* gamma, const float* beta,

@@ -12,14 +12,14 @@ def _declared_symbols():
     return sorted(set(re.findall(r"\b(cb_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_library_loads_and_exports_header_symbols():
+def test_library_loads_exports_header_symbols_and_abi_version():
     from celebbasis_b200 import lib
     L = lib.load()
     syms = _declared_symbols()
     assert len(syms) >= 35
     for s in syms:
         assert hasattr(L, s), f"symbol {s} declared in the header but not exported"
-    assert L.cb_abi_version() == 5
+    assert L.cb_abi_version() == 6
     assert isinstance(lib.last_error(), str)
 
 

@@ -125,17 +125,20 @@ def test_attention_fwd_bwd(dev, nq, nk, dh, heads, images):
 
 
 # ---------------------------------------------------------------------------------------------------- norms
-@pytest.mark.parametrize("n,hw,c,silu,eps,xdt", [(1, 4096, 320, True, 1e-5, torch.float32), (2, 64, 1280, True, 1e-5, torch.float32),
-                                                 (1, 1024, 960, False, 1e-6, torch.float32), (1, 4096, 128, True, 1e-6, torch.float16),
-                                                 (1, 1, 256, True, 1e-5, torch.float32),
-                                                 # cluster variant (slabs of groups, statistics through DSMEM): the UNet's 16^2 /
-                                                 # 8^2 concat widths, 30- and 10-channel groups (quads straddle two groups),
-                                                 # several images, fewer rows than cluster CTAs
-                                                 (1, 256, 2560, True, 1e-5, torch.float32), (1, 64, 1280, True, 1e-5, torch.float16),
-                                                 (1, 1024, 1920, True, 1e-5, torch.float32), (4, 64, 320, False, 1e-5, torch.float32),
-                                                 (1, 4096, 640, True, 1e-5, torch.float16), (3, 9, 960, True, 1e-6, torch.float32),
-                                                 # larger than the SMs' shared memory: TMA-streamed two-kernel path (VAE maps)
-                                                 (1, 65536, 128, True, 1e-6, torch.float32), (2, 20001, 256, False, 1e-6, torch.float16)])
+@pytest.mark.parametrize("n,hw,c,silu,eps,xdt", [
+    # forward and backward on the cluster kernels (slabs of groups, statistics through DSMEM)
+    (1, 4096, 320, True, 1e-5, torch.float32), (2, 64, 1280, True, 1e-5, torch.float32),
+    (1, 1024, 960, False, 1e-6, torch.float32), (1, 4096, 128, True, 1e-6, torch.float16),
+    (1, 1, 256, True, 1e-5, torch.float32),
+    # also both on the cluster kernels: the UNet's 16^2 / 8^2 concat widths, 30- and 10-channel groups (quads straddle two
+    # groups), several images, fewer rows than cluster CTAs
+    (1, 256, 2560, True, 1e-5, torch.float32), (1, 64, 1280, True, 1e-5, torch.float16),
+    (1, 1024, 1920, True, 1e-5, torch.float32), (4, 64, 320, False, 1e-5, torch.float32),
+    (1, 4096, 640, True, 1e-5, torch.float16), (3, 9, 960, True, 1e-6, torch.float32),
+    # a VAE 256^2 map: forward on the TMA-streamed statistics + apply pair, backward on the statistics + apply pair
+    (1, 65536, 128, True, 1e-6, torch.float32),
+    # forward on the cluster kernel (16-bit x fits), backward (x and dy staged) on the statistics + apply pair
+    (2, 20001, 256, False, 1e-6, torch.float16)])
 def test_groupnorm_fwd_bwd(dev, n, hw, c, silu, eps, xdt):
     from celebbasis_b200 import ops
     x = rnd(n * hw, c, dtype=xdt, scale=2.0) + 0.5
@@ -442,7 +445,8 @@ def test_gemm_tile256(dev):
 
 def test_groupnorm_bwd_emits_16bit_copy(dev):
     from celebbasis_b200 import ops
-    for (hw, c) in ((32, 640), (128, 128)):          # fused single-kernel path / streaming two-kernel path
+    # fp32 x, fp16 dy: the backward runs on the cluster kernel / on the statistics + apply pair
+    for (hw, c) in ((32, 640), (256, 128)):
         geo = ops.Geo(1, hw, hw)
         x = rnd(geo.rows, c, dtype=torch.float32, scale=2.0)
         gm, bt = rnd(c, dtype=torch.float32) * 0.1 + 1, rnd(c, dtype=torch.float32) * 0.1

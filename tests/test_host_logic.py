@@ -157,10 +157,11 @@ def test_gemm_autotune_key_and_lanes():
     assert ops._LANE == 0
 
 
-def test_gemm_tuned_config_dispatch_per_lane(monkeypatch):
+def test_gemm_config_and_groupnorm_flags_per_lane(monkeypatch):
     """The autotuner's winner reaches cb_gemm through the descriptor; a winner that launches a cluster of k-slices
     (splitk_cluster) is only used on the lane-0 stream -- other lanes take the best non-cluster configuration -- and the
-    front-end SM budget turns large lane-2 GEMMs into capped CTA-pair launches (no GPU: cb_gemm is a recording stub)."""
+    front-end SM budget turns large lane-2 GEMMs into capped CTA-pair launches (no GPU: cb_gemm is a recording stub) and
+    caps the lane-2 GroupNorm's CTAs through its flag word (SiLU in bit 0, CB_GN_CTA_CAP(n) in bits 8..23)."""
     import torch
     from celebbasis_b200 import ops
     from celebbasis_b200.lib import GemmDesc
@@ -220,14 +221,17 @@ def test_gemm_tuned_config_dispatch_per_lane(monkeypatch):
     assert seen[-1] == (0, 0, 0, 0, 0)
     assert ops._gn_flags(True) == 1
     with ops.lane(2):
-        assert ops._gn_flags(True) == (1 | 2 | (64 << 8))    # SiLU | no grid barrier | CB_GN_CTA_CAP(64)
+        assert ops._gn_flags(True) == (1 | (64 << 8))        # SiLU | CB_GN_CTA_CAP(64)
 
 
 def test_groupnorm_cluster_plan_covers_the_step():
     """cb_groupnorm_cluster_plan (host-only entry point of the library): every GroupNorm of the bs=1 SD-v1 UNet step --
     forward (fp32 or 16-bit input) and backward (input + 16-bit gradient staged) -- runs on the cluster variant: 128 CTAs as
     8 slabs x 16, staged rows within 200 KiB; each CTA's thread map (4-channel accesses, row lanes) touches every element of
-    its rows x slab exactly once; tensors that do not fit (VAE 512^2 maps, a 16-image UNet batch) report 0."""
+    its rows x slab exactly once; tensors that do not fit (VAE 512^2 maps, a 16-image UNet batch) report 0.  The route of
+    every forward of the VAE encoder (bs=1), the txt2img UNet (16 images: classifier-free guidance at batch 8) and the VAE
+    decoder (1 and 8 images) is pinned, and every shape without a plan has the 16-byte rows the streaming pair needs;
+    cb_groupnorm_fwd refuses other rows before any launch."""
     import ctypes
     import numpy as np
     from celebbasis_b200 import lib
@@ -265,6 +269,26 @@ def test_groupnorm_cluster_plan_covers_the_step():
     assert ask(1, 512 * 512, 128, 4) is None and ask(16, 4096, 320, 4) is None and ask(2, 4096, 960, 4) is None
     assert ask(2, 4096, 320, 4)[0] == 8 and ask(4, 64, 320, 4)[0] == 4 and ask(1, 1, 256, 4)[0] == 1
     assert L.cb_groupnorm_cluster_plan(1, 64, 48, 32, 4, ctypes.cast(plan, ctypes.c_void_p)) < 0      # odd channels per group
+    enc = [(512 * 512, 128), (256 * 256, 128), (256 * 256, 256), (128 * 128, 256), (128 * 128, 512), (64 * 64, 512)]
+    dec = [(64 * 64, 512), (128 * 128, 512), (256 * 256, 512), (256 * 256, 256), (512 * 512, 256), (512 * 512, 128)]
+    # (images, (HW, C) shapes, the (HW, C, sizeof(x)) forwards that take the cluster kernel); x is fp32 or 16-bit
+    routes = [
+        (1, enc, {(256 * 256, 128, 2), (128 * 128, 256, 4), (128 * 128, 256, 2), (128 * 128, 512, 2), (64 * 64, 512, 4),
+                  (64 * 64, 512, 2)}),
+        (16, unet, {(4096, 320, 2), (1024, 320, 4), (1024, 320, 2), (1024, 640, 4), (1024, 640, 2), (1024, 960, 2),
+                    (1024, 1280, 2)} | {(hw, c, bpe) for hw, c in unet if hw <= 256 for bpe in (4, 2)}),
+        (1, dec, {(64 * 64, 512, 4), (64 * 64, 512, 2), (128 * 128, 512, 2)}),
+        (8, dec, {(64 * 64, 512, 2)}),
+    ]
+    for N, shapes, cluster in routes:
+        for hw, c in shapes:
+            for bpe in (4, 2):
+                assert (ask(N, hw, c, bpe) is not None) == ((hw, c, bpe) in cluster), (N, hw, c, bpe)
+                assert (hw, c, bpe) in cluster or c * bpe % 16 == 0, (N, hw, c, bpe)    # the streaming pair's rows
+    # rows that are not a multiple of 16 bytes (G = 3, C = 6, fp16: 12-byte rows): refused before anything is launched
+    assert L.cb_groupnorm_fwd(None, lib.CB_F16, None, lib.CB_F16, None, None, 1, 16, 6, 3, 1e-5, 0, None, None, None,
+                              None) < 0
+    assert b"16 bytes" in L.cb_last_error()
 
 
 def test_bench_reference_arm_contract():

@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B of the cluster GroupNorm (default on) and the cluster split-K variants on one box; every leg under its own hard timeout
+# A/B of the cluster split-K variants on one box; every leg under its own hard timeout
 # (a hung leg must not take the rest of the call with it).  Outputs under tools_out/.
 T=${1:-r02e}
 O=tools_out
@@ -10,6 +10,5 @@ run() {   # name, env assignments...
     echo "$name rc=$? $(cut -c1-230 $O/${T}_bench_${name}.json)"
 }
 run default CB_NOOP=1
-run gn_cluster_off CB_GN_CLUSTER=0
 run cluster_sk_lane0 CB_GEMM_CLUSTER_SK=1
 run cluster_sk_all CB_GEMM_CLUSTER_SK=2

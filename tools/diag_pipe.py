@@ -46,4 +46,4 @@ torch.cuda.synchronize()
 print("VAE alone lane2: z", rel(zz, z1))
 zz0, _ = eng.encode_first_stage(G.image_n, G.peps_n)
 torch.cuda.synchronize()
-print("VAE alone lane0 (fused GN): z", rel(zz0, z1))
+print("VAE alone lane0: z", rel(zz0, z1))

@@ -1,10 +1,17 @@
-"""Bisect the fused GroupNorm kernel's time (CB_GN_DBG bits: 1 no grid barrier, 2 no fold, 4 no staging load, 8 return after load)."""
-import os, sys
+"""Per-node time of GroupNorm forward / backward at the UNet and VAE shapes (CUDA-graph replay), labelled with the route
+each call takes: "cluster" (one launch) or "pair" (statistics + apply launches)."""
+import ctypes, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
-from celebbasis_b200 import ops
+from celebbasis_b200 import lib, ops
 dev = torch.device("cuda:0")
+_plan = (ctypes.c_int32 * 4)()
+
+
+def route(N, HW, C, bytes_per_elem):
+    rc = lib.load().cb_groupnorm_cluster_plan(N, HW, C, 32, bytes_per_elem, ctypes.cast(_plan, ctypes.c_void_p))
+    return "cluster" if rc == 1 else "pair"
 
 def per_node(name, fn, n=100):
     fn(); torch.cuda.synchronize()
@@ -21,18 +28,15 @@ def per_node(name, fn, n=100):
     print(f"{name}: {e0.elapsed_time(e1) * 1000 / (5 * n):.2f} us per node", flush=True)
 
 xn = torch.randn(4096, 320, device=dev); gm = torch.ones(320, device=dev); bt = torch.zeros(320, device=dev)
-y = None
-for dbg in (0,):
-    os.environ["CB_GN_DBG"] = str(dbg)
-    per_node(f"groupnorm 4096x320 dbg={dbg}", lambda: ops.groupnorm(xn, ops.Geo(1, 64, 64), gm, bt))
+per_node(f"groupnorm 4096x320 [{route(1, 4096, 320, 4)}]", lambda: ops.groupnorm(xn, ops.Geo(1, 64, 64), gm, bt))
 for (hw, c) in ((64, 320), (64, 640), (32, 640), (32, 1280), (16, 1280), (16, 2560), (8, 1280), (8, 2560), (64, 960)):
     xs = torch.randn(hw * hw, c, device=dev); g2 = torch.ones(c, device=dev); b2 = torch.zeros(c, device=dev)
-    per_node(f"groupnorm+silu {hw}x{hw}x{c}", lambda: ops.groupnorm(xs, ops.Geo(1, hw, hw), g2, b2, silu=True))
+    per_node(f"groupnorm+silu {hw}x{hw}x{c} [{route(1, hw * hw, c, 4)}]", lambda: ops.groupnorm(xs, ops.Geo(1, hw, hw), g2, b2, silu=True))
     y, stt = ops.groupnorm(xs, ops.Geo(1, hw, hw), g2, b2, silu=True)
     dy = torch.randn(hw * hw, c, device=dev).half()
-    per_node(f"groupnorm_bwd      {hw}x{hw}x{c}", lambda: ops.groupnorm_bwd(dy, xs, ops.Geo(1, hw, hw), g2, b2, stt, silu=True))
+    per_node(f"groupnorm_bwd  {hw}x{hw}x{c} [{route(1, hw * hw, c, 4 + 2)}]", lambda: ops.groupnorm_bwd(dy, xs, ops.Geo(1, hw, hw), g2, b2, stt, silu=True))
 
-# VAE-size tensors (two-kernel path: statistics + apply)
+# VAE-size tensors
 for (hw, c, dt) in ((512, 128, torch.float32), (256, 256, torch.float32), (256, 128, torch.float32), (128, 512, torch.float32), (128, 256, torch.float32)):
     xs = torch.randn(hw * hw, c, device=dev).to(dt); g2 = torch.ones(c, device=dev); b2 = torch.zeros(c, device=dev)
-    per_node(f"groupnorm+silu 2-kernel {hw}x{hw}x{c} {str(dt)[6:]}", lambda: ops.groupnorm(xs, ops.Geo(1, hw, hw), g2, b2, silu=True), n=10)
+    per_node(f"groupnorm+silu {hw}x{hw}x{c} {str(dt)[6:]} [{route(1, hw * hw, c, 4)}]", lambda: ops.groupnorm(xs, ops.Geo(1, hw, hw), g2, b2, silu=True), n=10)

@@ -32,5 +32,5 @@ x3, w3 = rnd(4096, 320), rnd(2560, 320); o3 = torch.empty(4096, 2560, dtype=torc
 per_node("linear 4096x2560x320 (512 CTAs)", lambda: ops.linear(x3, w3, out=o3))
 xn = torch.randn(4096, 320, device=dev); gm = torch.ones(320, device=dev); bt = torch.zeros(320, device=dev)
 per_node("layernorm 4096x320", lambda: ops.layernorm(xn, gm, bt))
-per_node("groupnorm 4096x320 (fused, 1 kernel)", lambda: ops.groupnorm(xn, ops.Geo(1, 64, 64), gm, bt))
+per_node("groupnorm 4096x320 (cluster, 1 kernel)", lambda: ops.groupnorm(xn, ops.Geo(1, 64, 64), gm, bt))
 per_node("torch add (reference point)", lambda: torch.add(a, 1.0, out=b))

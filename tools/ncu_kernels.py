@@ -1,6 +1,6 @@
 """One launch each of the hot kernels between cudaProfilerStart/Stop (for `ncu --set full --profile-from-start off`):
 implicit-GEMM conv (UNet 64x64 320->320, VAE 128x128 512->512), a projection GEMM, flash attention forward and the two
-backward kernels at the UNet's 4096-token / 1024-token self-attention shapes, fused GroupNorm fwd/bwd."""
+backward kernels at the UNet's 4096-token / 1024-token self-attention shapes, cluster GroupNorm(+SiLU) fwd/bwd."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
