@@ -240,6 +240,47 @@ __global__ void q_sample_kernel(const float* __restrict__ x0, const float* __res
     }
 }
 
+// Masked DDIM blend before a step (ddim.py:144-147 around ddpm.py:289-292), one (b, c) row of HW pixels per blockIdx.y:
+//   img_orig = sqrt_ac[t_b]*x0 + sqrt_1mac[t_b]*noise;  out = img_orig*m + (1-m)*img
+// every operation is an explicitly rounded fp32 op in the reference's evaluation order (no FMA contraction), so the
+// result is bit-identical to the eager fp32 expression.  The mask row is mask + b*mask_sb + c*mask_sc (a stride of 0
+// broadcasts); `out` may alias `img` (each element is read before it is written, by the same thread).
+__device__ __forceinline__ float masked_blend(float a, float s, float x0, float nz, float m, float im) {
+    const float orig = __fadd_rn(__fmul_rn(a, x0), __fmul_rn(s, nz));
+    return __fadd_rn(__fmul_rn(orig, m), __fmul_rn(__fsub_rn(1.f, m), im));
+}
+
+template <bool kVec>
+__global__ void q_sample_masked_kernel(const float* __restrict__ x0, const float* __restrict__ noise,
+                                       const long long* __restrict__ t, const float* __restrict__ sqrt_ac,
+                                       const float* __restrict__ sqrt_1mac, const float* __restrict__ mask,
+                                       long long mask_sb, long long mask_sc, const float* img, float* out, int C,
+                                       int HW) {
+    pdl_sync();
+    const int b = blockIdx.y / C, c = blockIdx.y % C;
+    const float a = sqrt_ac[t[b]], s = sqrt_1mac[t[b]];
+    const size_t row = (size_t)blockIdx.y * HW;
+    const float* mrow = mask + b * mask_sb + c * mask_sc;
+    if (kVec) {
+        const int n4 = HW >> 2;
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+            const float4 xv = reinterpret_cast<const float4*>(x0 + row)[i];
+            const float4 nv = reinterpret_cast<const float4*>(noise + row)[i];
+            const float4 mv = reinterpret_cast<const float4*>(mrow)[i];
+            const float4 iv = reinterpret_cast<const float4*>(img + row)[i];
+            float4 o;
+            o.x = masked_blend(a, s, xv.x, nv.x, mv.x, iv.x);
+            o.y = masked_blend(a, s, xv.y, nv.y, mv.y, iv.y);
+            o.z = masked_blend(a, s, xv.z, nv.z, mv.z, iv.z);
+            o.w = masked_blend(a, s, xv.w, nv.w, mv.w, iv.w);
+            reinterpret_cast<float4*>(out + row)[i] = o;
+        }
+    } else {
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x)
+            out[row + i] = masked_blend(a, s, x0[row + i], noise[row + i], mrow[i], img[row + i]);
+    }
+}
+
 // DDIM update with classifier-free guidance (ldm/models/diffusion/ddim.py:166-204)
 __global__ void ddim_step_kernel(const float* __restrict__ x, const float* __restrict__ e_u, const float* __restrict__ e_c,
                                  const float* __restrict__ noise, float* __restrict__ x_prev, float* __restrict__ pred_x0,
@@ -299,6 +340,34 @@ extern "C" int cb_q_sample(const float* x0, const float* noise, const long long*
     CB_REQUIRE(B > 0 && per_sample > 0, CB_ERR_ARG, "q_sample: bad shape");
     dim3 grid((unsigned)((per_sample + 255) / 256 > 64 ? 64 : (per_sample + 255) / 256), (unsigned)B);
 CB_LAUNCH((q_sample_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), x0, noise, t, sqrt_ac, sqrt_1mac, out, per_sample);
+    CB_CUDA(cudaGetLastError());
+    cb::count_launches(1);
+    return 0;
+}
+
+extern "C" int cb_q_sample_masked(const float* x0, const float* noise, const long long* t, const float* sqrt_ac,
+                                  const float* sqrt_1mac, const float* mask, long long mask_bstride,
+                                  long long mask_cstride, const float* img, float* out, int B, int C, int HW,
+                                  void* stream) {
+    CB_REQUIRE(x0 && noise && t && sqrt_ac && sqrt_1mac && mask && img && out, CB_ERR_ARG,
+               "q_sample_masked: NULL pointer");
+    CB_REQUIRE(B > 0 && C > 0 && HW > 0 && (long long)B * C <= 65535, CB_ERR_ARG, "q_sample_masked: bad shape");
+    CB_REQUIRE(mask_bstride >= 0 && mask_cstride >= 0, CB_ERR_ARG,
+               "q_sample_masked: mask strides must be >= 0 (0 = broadcast)");
+    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    const bool vec = HW % 4 == 0 && mask_bstride % 4 == 0 && mask_cstride % 4 == 0 && al16(x0) && al16(noise) &&
+                     al16(mask) && al16(img) && al16(out);
+    const int per_block = 256 * (vec ? 4 : 1);
+    int bx = (HW + per_block - 1) / per_block;
+    if (bx > 64) bx = 64;
+    dim3 grid((unsigned)bx, (unsigned)(B * C));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (vec)
+        CB_LAUNCH((q_sample_masked_kernel<true>), grid, 256, 0, st, x0, noise, t, sqrt_ac, sqrt_1mac, mask,
+                  mask_bstride, mask_cstride, img, out, C, HW);
+    else
+        CB_LAUNCH((q_sample_masked_kernel<false>), grid, 256, 0, st, x0, noise, t, sqrt_ac, sqrt_1mac, mask,
+                  mask_bstride, mask_cstride, img, out, C, HW);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
     return 0;

@@ -509,10 +509,11 @@ class LatentDiffusion(DDPM):
     def log_images(self, batch, N=8, n_row=4, sample=True, ddim_steps=50, ddim_eta=1., return_keys=None,
                    quantize_denoised=True, inpaint=False, plot_denoise_rows=False, plot_progressive_rows=False,
                    plot_diffusion_rows=False, **kwargs):
-        """inputs / reconstruction / rendered captions / DDIM samples (plain and with guidance 5.0), as the reference logs
-        them (the inpainting, progressive and diffusion-row panels are off in every CelebBasis config)."""
+        """inputs / reconstruction / rendered captions / DDIM samples (plain and with guidance 5.0) and, with inpaint, the
+        masked-sampling panels, as the reference logs them (the progressive, denoise-row and diffusion-row panels are off
+        in every CelebBasis config)."""
         from ldm.util import log_txt_as_img
-        assert not (inpaint or plot_denoise_rows or plot_progressive_rows or plot_diffusion_rows)
+        assert not (plot_denoise_rows or plot_progressive_rows or plot_diffusion_rows)
         batch = self.preprocess_batch(batch)
         log = dict()
         z, c, x, xrec, xc = self.get_input(batch, self.first_stage_key, return_first_stage_outputs=True,
@@ -533,6 +534,22 @@ class LatentDiffusion(DDPM):
                                                eta=ddim_eta, unconditional_guidance_scale=5.0,
                                                unconditional_conditioning=uc)
             log["samples_scaled"] = self.decode_first_stage(sample_scaled)
+            if inpaint:
+                # ddpm.py:1405-1425: keep the latent outside a centre square; the reference passes the SAME mask to its
+                # outpainting call, so both panels sample the square
+                h, w = z.shape[2], z.shape[3]
+                mask = torch.ones(N, h, w, device=z.device)
+                mask[:, h // 4:3 * h // 4, w // 4:3 * w // 4] = 0.
+                mask = mask[:, None, ...]
+                with self.ema_scope("Plotting Inpaint"):
+                    samples, _ = self.sample_log(cond=c, batch_size=N, ddim=ddim_steps is not None, eta=ddim_eta,
+                                                 ddim_steps=ddim_steps, x0=z[:N], mask=mask)
+                log["samples_inpainting"] = self.decode_first_stage(samples)
+                log["mask"] = mask
+                with self.ema_scope("Plotting Outpaint"):
+                    samples, _ = self.sample_log(cond=c, batch_size=N, ddim=ddim_steps is not None, eta=ddim_eta,
+                                                 ddim_steps=ddim_steps, x0=z[:N], mask=mask)
+                log["samples_outpainting"] = self.decode_first_stage(samples)
         if return_keys:
             if np.intersect1d(list(log.keys()), return_keys).shape[0] == 0:
                 return log

@@ -765,6 +765,29 @@ def q_sample(x0, noise, t, sqrt_ac, sqrt_1mac):
     return out
 
 
+def mask_strides(mask, shape):
+    """(batch stride, channel stride) of an fp32 mask broadcast to `shape` = (B, C, h, w), 0 where it broadcasts.  The
+    spatial dimensions must be dense (stride w and 1)."""
+    B, C, h, w = shape
+    sb, sc, sh, sw = mask.expand(B, C, h, w).stride()
+    if (h > 1 and sh != w) or (w > 1 and sw != 1):
+        raise ValueError(f"mask of shape {tuple(mask.shape)} / strides {tuple(mask.stride())}: spatial dims must be dense")
+    return (sb if B > 1 else 0), (sc if C > 1 else 0)
+
+
+def q_sample_masked(x0, noise, t, sqrt_ac, sqrt_1mac, mask, img, out=None):
+    """out = q_sample(x0, t, noise) * mask + (1 - mask) * img (ddim.py:144-147) in one launch; `out` may be `img`."""
+    B, C, h, w = img.shape
+    assert x0.shape == noise.shape == img.shape and mask.dtype == torch.float32
+    assert x0.is_contiguous() and noise.is_contiguous() and img.is_contiguous() and t.dtype == torch.long
+    sb, sc = mask_strides(mask, (B, C, h, w))
+    out = torch.empty_like(img) if out is None else out
+    assert out.shape == img.shape and out.is_contiguous()
+    _lib.check(_L().cb_q_sample_masked(_p(x0), _p(noise), _p(t), _p(sqrt_ac), _p(sqrt_1mac), _p(mask), sb, sc, _p(img),
+                                       _p(out), B, C, h * w, _st()), "cb_q_sample_masked")
+    return out
+
+
 def ddim_step(x, e_uncond, e_cond, noise, *, scale, a_t, a_prev, sigma_t, sqrt_one_minus_at, want_x0=True):
     x_prev = torch.empty_like(x)
     pred_x0 = torch.empty_like(x) if want_x0 else None

@@ -295,6 +295,15 @@ int cb_ddim_step(const float* x, const float* e_uncond, const float* e_cond, con
 /* cb_q_sample: DDPM.q_sample (ddpm.py:289-292) with the timestep read on the device: out = sqrt_ac[t]*x0 + sqrt_1mac[t]*noise */
 int cb_q_sample(const float* x0, const float* noise, const long long* t, const float* sqrt_ac, const float* sqrt_1mac,
                 float* out, int B, int per_sample, void* stream);
+/* cb_q_sample_masked: the inpainting / outpainting blend DDIMSampler.ddim_sampling applies before every step when a mask
+ *   is given (ddim.py:144-147), with DDPM.q_sample (ddpm.py:289-292) fused in; x0, noise, img, out are [B][C][HW] fp32:
+ *     out = (sqrt_ac[t_b]*x0 + sqrt_1mac[t_b]*noise) * m + (1 - m) * img,   m = mask[b*mask_bstride + c*mask_cstride + p]
+ *   t is read on the device (int64, B entries).  The fp32 mask's spatial dimensions are dense; a batch or channel stride
+ *   of 0 broadcasts that dimension ((B,1,h,w), (1,1,h,w) and (B,C,h,w) masks; soft values allowed).  out may alias img.
+ *   Each operation is rounded separately, in the reference's order: bit-identical to the eager fp32 expression. */
+int cb_q_sample_masked(const float* x0, const float* noise, const long long* t, const float* sqrt_ac,
+                       const float* sqrt_1mac, const float* mask, long long mask_bstride, long long mask_cstride,
+                       const float* img, float* out, int B, int C, int HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * CosFace-R100 front end (no-grad): meta_net.py:253-264, iresnet.py:26-64.
