@@ -838,7 +838,9 @@ static int pick_bn(const cb_gemm_desc& d, int m_tiles, int kiters, bool requeste
     }
     static const int env_bn = getenv("CB_GEMM_BN") ? atoi(getenv("CB_GEMM_BN")) : 0;   // tuning aid
     const int force_bn = !requested ? 0 : (d.tile_n > 0 ? d.tile_n : env_bn);
-    if (force_bn == 256 && N >= 256) return 256;    // 128x256 tile: only on request (per-shape autotuner / caller)
+    // 128x256 tile: only on request (per-shape autotuner / caller), and only with K-major A -- there is no MN-major-A
+    // instantiation of that width, so such a request falls through to the model below
+    if (force_bn == 256 && N >= 256 && d.a_major != CB_MAJOR_MN) return 256;
     for (int i = 0; i < nc; ++i)
         if (cands[i] == force_bn) return force_bn;
     int best = cands[0];

@@ -139,7 +139,8 @@ typedef struct cb_gemm_desc {
      * {start, setup done, first stage full, last MMA issued, accumulator ready, exit, 4th stage full, -}. */
     void* debug_timeline;
 
-    /* tuning overrides, 0 = the library's cost model: tile width (64 / 128 / 160 / 256; 160 only with K-major B) and the
+    /* tuning overrides, 0 = the library's cost model: tile width (64 / 128 / 160 / 256; 160 only with K-major B, 256 only
+     * with K-major A and N >= 256; a width the operand majors do not allow is ignored) and the
      * number of split-K slices (1 = no split; ignored when the workspace cannot hold it).  Without a splits request
      * the split count depends on the shape only, never on tile_n / stages / cta_pair / splitk_cluster, so those knobs
      * do not change the results.  The host autotuner (celebbasis_b200/ops.py) times them once per shape and passes the
