@@ -474,15 +474,28 @@ using namespace cb;
     else if ((dtype) == CB_BF16) { using T = __nv_bfloat16; __VA_ARGS__; }       \
     else { cb::set_error("dtype %d must be f16/bf16", (int)(dtype)); return CB_ERR_ARG; }
 
+// element size of a CB_F16 / CB_BF16 / CB_F32 code, 0 for any other code
+static inline int dt_size(int dt) { return dt == CB_F32 ? 4 : (dt == CB_F16 || dt == CB_BF16) ? 2 : 0; }
+static inline bool act_ok(int act) {
+    return act == CB_ACT_NONE || act == CB_ACT_SILU || act == CB_ACT_GELU || act == CB_ACT_QUICK_GELU;
+}
+// the V4 accesses move 4 elements at once: 16 B for fp32, 8 B for the 16-bit types
+static inline bool vec4_aligned(const void* p, int dt) {
+    return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(4 * dt_size(dt) - 1)) == 0;
+}
+
 extern "C" int cb_axpby2d(const void* x, int x_dtype, long long ldx, float a, const void* y, int y_dtype,
                           long long ldy, float b, void* out, int o_dtype, long long ldo, long long rows, int cols,
                           void* stream) {
     CB_REQUIRE(rows > 0 && cols > 0 && cols % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0 && (y == nullptr || ldy % 4 == 0),
                CB_ERR_ARG, "axpby2d: cols/ld must be multiples of 4 (rows=%lld cols=%d)", rows, cols);
+    if (y == nullptr) y_dtype = x_dtype;
+    CB_REQUIRE(dt_size(x_dtype) && dt_size(y_dtype) && dt_size(o_dtype), CB_ERR_ARG, "axpby2d: unsupported dtype");
+    CB_REQUIRE(vec4_aligned(x, x_dtype) && (y == nullptr || vec4_aligned(y, y_dtype)) && vec4_aligned(out, o_dtype),
+               CB_ERR_ALIGN, "axpby2d: x, y and out must be aligned to 4 elements");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int c4 = cols / 4;
     const int grid = grid_for(rows * c4, 256);
-    if (y == nullptr) y_dtype = x_dtype;
     CB_DISPATCH(x_dtype, TX, CB_DISPATCH(y_dtype, TY, CB_DISPATCH(o_dtype, TO,
 CB_LAUNCH((axpby2d_kernel<TX, TY, TO>), grid, 256, 0, st, (const TX*)x, ldx, a, (const TY*)y, ldy, b, (TO*)out, ldo, rows, c4))));
     CB_CUDA(cudaGetLastError());
@@ -492,6 +505,7 @@ CB_LAUNCH((axpby2d_kernel<TX, TY, TO>), grid, 256, 0, st, (const TX*)x, ldx, a, 
 
 extern "C" int cb_act_fwd(const void* x, int x_dtype, void* y, int y_dtype, long long n, int act, void* stream) {
     CB_REQUIRE(n > 0, CB_ERR_ARG, "act_fwd: n<=0");
+    CB_REQUIRE(dt_size(x_dtype) && dt_size(y_dtype) && act_ok(act), CB_ERR_ARG, "act_fwd: unsupported dtype or act %d", act);
 CB_LAUNCH((act_fwd_kernel), grid_for(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), x, x_dtype, y, y_dtype, (size_t)n, act);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
@@ -500,6 +514,8 @@ CB_LAUNCH((act_fwd_kernel), grid_for(n, 256), 256, 0, reinterpret_cast<cudaStrea
 extern "C" int cb_act_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, void* dx, int dx_dtype,
                           long long n, int act, void* stream) {
     CB_REQUIRE(n > 0, CB_ERR_ARG, "act_bwd: n<=0");
+    CB_REQUIRE(dt_size(dy_dtype) && dt_size(x_dtype) && dt_size(dx_dtype) && act_ok(act), CB_ERR_ARG,
+               "act_bwd: unsupported dtype or act %d", act);
 CB_LAUNCH((act_bwd_kernel), grid_for(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), dy, dy_dtype, x, x_dtype, dx, dx_dtype, (size_t)n, act);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
@@ -507,7 +523,10 @@ CB_LAUNCH((act_bwd_kernel), grid_for(n, 256), 256, 0, reinterpret_cast<cudaStrea
 }
 
 extern "C" int cb_geglu_fwd(const void* in, void* out, int dtype, long long M, int F, int interleave, void* stream) {
-    CB_REQUIRE(M > 0 && F > 0 && F % 4 == 0, CB_ERR_ARG, "geglu_fwd: bad shape");
+    CB_REQUIRE(M > 0 && F > 0 && F % (interleave ? 32 : 4) == 0, CB_ERR_ARG, "geglu_fwd: bad shape");
+    CB_REQUIRE(dt_size(dtype) == 2, CB_ERR_ARG, "geglu_fwd: dtype %d must be f16/bf16", dtype);
+    CB_REQUIRE(vec4_aligned(in, dtype) && vec4_aligned(out, dtype), CB_ERR_ALIGN,
+               "geglu_fwd: in and out must be 8-byte aligned");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CB_DISPATCH16(dtype, T,CB_LAUNCH((geglu_fwd_kernel<T>), grid_for(M * (F / 4), 256), 256, 0, st, (const T*)in, (T*)out, M, F, interleave));
     CB_CUDA(cudaGetLastError());
@@ -516,7 +535,10 @@ extern "C" int cb_geglu_fwd(const void* in, void* out, int dtype, long long M, i
 }
 extern "C" int cb_geglu_bwd(const void* dout, const void* in, void* din, int dtype, int g_dtype, long long M, int F,
                             int interleave, void* stream) {
-    CB_REQUIRE(M > 0 && F > 0 && F % 4 == 0, CB_ERR_ARG, "geglu_bwd: bad shape");
+    CB_REQUIRE(M > 0 && F > 0 && F % (interleave ? 32 : 4) == 0, CB_ERR_ARG, "geglu_bwd: bad shape");
+    CB_REQUIRE(dt_size(dtype) == 2 && dt_size(g_dtype) == 2, CB_ERR_ARG, "geglu_bwd: dtypes must be f16/bf16");
+    CB_REQUIRE(vec4_aligned(dout, g_dtype) && vec4_aligned(in, dtype) && vec4_aligned(din, g_dtype), CB_ERR_ALIGN,
+               "geglu_bwd: dout, in and din must be 8-byte aligned");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CB_DISPATCH16(dtype, T, CB_DISPATCH16(g_dtype, TG,
 CB_LAUNCH((geglu_bwd_kernel<T, TG>), grid_for(M * (F / 4), 256), 256, 0, st, (const TG*)dout, (const T*)in, (TG*)din, M, F, interleave)));
@@ -547,6 +569,9 @@ CB_LAUNCH((softmax_bwd_kernel<T, TG>), (unsigned)rows, 128, 0, st, (const TG*)dp
 
 extern "C" int cb_upsample2x_fwd(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream) {
     CB_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, CB_ERR_ARG, "upsample2x_fwd: bad shape");
+    CB_REQUIRE(dt_size(dtype), CB_ERR_ARG, "upsample2x_fwd: unsupported dtype %d", dtype);
+    CB_REQUIRE(vec4_aligned(x, dtype) && vec4_aligned(y, dtype), CB_ERR_ALIGN,
+               "upsample2x_fwd: x and y must be aligned to 4 elements");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long total = (long long)N * 4 * H * W * (C / 4);
     CB_DISPATCH(dtype, T,CB_LAUNCH((upsample2x_fwd_kernel<T>), grid_for(total, 256), 256, 0, st, (const T*)x, (T*)y, N, H, W, C / 4));
@@ -557,6 +582,9 @@ extern "C" int cb_upsample2x_fwd(const void* x, void* y, int dtype, int N, int H
 extern "C" int cb_upsample2x_bwd(const void* dy, int dy_dtype, void* dx, int dx_dtype, int N, int H, int W, int C,
                                  int accumulate, void* stream) {
     CB_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, CB_ERR_ARG, "upsample2x_bwd: bad shape");
+    CB_REQUIRE(dt_size(dy_dtype) && dt_size(dx_dtype), CB_ERR_ARG, "upsample2x_bwd: unsupported dtype");
+    CB_REQUIRE(vec4_aligned(dy, dy_dtype) && vec4_aligned(dx, dx_dtype), CB_ERR_ALIGN,
+               "upsample2x_bwd: dy and dx must be aligned to 4 elements");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long total = (long long)N * H * W * (C / 4);
     CB_DISPATCH(dy_dtype, TG, CB_DISPATCH(dx_dtype, TD,
@@ -567,6 +595,9 @@ CB_LAUNCH((upsample2x_bwd_kernel<TG, TD>), grid_for(total, 256), 256, 0, st, (co
 }
 extern "C" int cb_zero_insert2x(const void* dy, void* z, int dtype, int N, int H, int W, int C, void* stream) {
     CB_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, CB_ERR_ARG, "zero_insert2x: bad shape");
+    CB_REQUIRE(dt_size(dtype), CB_ERR_ARG, "zero_insert2x: unsupported dtype %d", dtype);
+    CB_REQUIRE(vec4_aligned(dy, dtype) && vec4_aligned(z, dtype), CB_ERR_ALIGN,
+               "zero_insert2x: dy and z must be aligned to 4 elements");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long total = (long long)N * 4 * H * W * (C / 4);
     CB_DISPATCH(dtype, T,CB_LAUNCH((zero_insert2x_kernel<T>), grid_for(total, 256), 256, 0, st, (const T*)dy, (T*)z, N, H, W, C / 4));
@@ -577,6 +608,7 @@ extern "C" int cb_zero_insert2x(const void* dy, void* z, int dtype, int N, int H
 
 extern "C" int cb_nchw_to_nhwc(const float* x, void* y, int y_dtype, int N, int C, int HW, int Cpad, void* stream) {
     CB_REQUIRE(N > 0 && C > 0 && HW > 0 && Cpad >= C, CB_ERR_ARG, "nchw_to_nhwc: bad shape");
+    CB_REQUIRE(dt_size(y_dtype), CB_ERR_ARG, "nchw_to_nhwc: unsupported dtype %d", y_dtype);
 CB_LAUNCH((nchw_to_nhwc_kernel), grid_for((long long)N * HW * Cpad, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), x, y, y_dtype, N, C, HW, Cpad);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
@@ -584,6 +616,7 @@ CB_LAUNCH((nchw_to_nhwc_kernel), grid_for((long long)N * HW * Cpad, 256), 256, 0
 }
 extern "C" int cb_nhwc_to_nchw(const void* x, int x_dtype, float* y, int N, int C, int HW, int Cpad, void* stream) {
     CB_REQUIRE(N > 0 && C > 0 && HW > 0 && Cpad >= C, CB_ERR_ARG, "nhwc_to_nchw: bad shape");
+    CB_REQUIRE(dt_size(x_dtype), CB_ERR_ARG, "nhwc_to_nchw: unsupported dtype %d", x_dtype);
 CB_LAUNCH((nhwc_to_nchw_kernel), grid_for((long long)N * HW * C, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), x, x_dtype, y, N, C, HW, Cpad);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
@@ -604,6 +637,7 @@ extern "C" int cb_mse_fwd_bwd(const float* pred, const float* target, float* los
 extern "C" int cb_timestep_embedding(const long long* t, void* out, int o_dtype, int B, int dim, float max_period,
                                      void* stream) {
     CB_REQUIRE(B > 0 && dim >= 2, CB_ERR_ARG, "timestep_embedding: bad shape");
+    CB_REQUIRE(dt_size(o_dtype), CB_ERR_ARG, "timestep_embedding: unsupported dtype %d", o_dtype);
     const int n = B * (dim / 2);
 CB_LAUNCH((timestep_embedding_kernel), ceil_div(n, 128), 128, 0, reinterpret_cast<cudaStream_t>(stream), t, out, o_dtype, B, dim, max_period);
     CB_CUDA(cudaGetLastError());
@@ -614,6 +648,10 @@ CB_LAUNCH((timestep_embedding_kernel), ceil_div(n, 128), 128, 0, reinterpret_cas
 extern "C" int cb_channel_affine_act(const void* x, int x_dtype, void* y, int y_dtype, const float* scale,
                                      const float* shift, const float* slope, long long rows, int C, void* stream) {
     CB_REQUIRE(rows > 0 && C > 0 && C % 4 == 0, CB_ERR_ARG, "channel_affine_act: bad shape");
+    CB_REQUIRE((scale == nullptr) == (shift == nullptr), CB_ERR_ARG, "channel_affine_act: scale and shift go together");
+    CB_REQUIRE(dt_size(x_dtype) && dt_size(y_dtype), CB_ERR_ARG, "channel_affine_act: unsupported dtype");
+    CB_REQUIRE(vec4_aligned(x, x_dtype) && vec4_aligned(y, y_dtype), CB_ERR_ALIGN,
+               "channel_affine_act: x and y must be aligned to 4 elements");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CB_DISPATCH(x_dtype, T, CB_DISPATCH(y_dtype, TY,
 CB_LAUNCH((channel_affine_act_kernel<T, TY>), grid_for(rows * (C / 4), 256), 256, 0, st, (const T*)x, (TY*)y, scale, shift, slope, rows, C / 4)));
@@ -625,6 +663,7 @@ CB_LAUNCH((channel_affine_act_kernel<T, TY>), grid_for(rows * (C / 4), 256), 256
 extern "C" int cb_face_warp_resize(const float* faces, void* out, int o_dtype, int B, int H, int W, int n_chunks,
                                    int out_hw, int Cpad, const float* host_affine6, void* stream) {
     CB_REQUIRE(B > 0 && H > 1 && W > 1 && n_chunks > 0 && out_hw > 1 && Cpad >= 3 && host_affine6, CB_ERR_ARG, "face_warp_resize: bad args");
+    CB_REQUIRE(dt_size(o_dtype), CB_ERR_ARG, "face_warp_resize: unsupported dtype %d", o_dtype);
     const int total = n_chunks * B * out_hw * out_hw * Cpad;
 CB_LAUNCH((face_warp_resize_kernel), ceil_div(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), 
         faces, out, o_dtype, B, H, W, n_chunks, out_hw, Cpad, host_affine6[0], host_affine6[1], host_affine6[2],

@@ -187,13 +187,13 @@ __global__ void embed_inject_bwd_kernel(const float* __restrict__ dout, const in
 
 __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                              float* __restrict__ v, long long n, float lr, float b1, float b2, float eps, float wd,
-                             float bc1, float bc2_sqrt, const int* __restrict__ step_dev) {
+                             int step, const int* __restrict__ step_dev) {
     pdl_sync();
-    if (step_dev) {  // graph-replay friendly: the step counter lives on the device
-        const float t = (float)(*step_dev + 1);
-        bc1 = 1.f - powf(b1, t);
-        bc2_sqrt = sqrtf(1.f - powf(b2, t));
-    }
+    // graph-replay friendly: with step_dev the step counter lives on the device.  The bias corrections are formed here
+    // for both paths, so a host-counted and a device-counted run produce the same bits.
+    const float t = (float)(step_dev ? *step_dev + 1 : step);
+    const float bc1 = 1.f - powf(b1, t);
+    const float bc2_sqrt = sqrtf(1.f - powf(b2, t));
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const float gi = g[i];
         float pi = p[i] * (1.f - lr * wd);
@@ -376,6 +376,8 @@ extern "C" int cb_q_sample_masked(const float* x0, const float* noise, const lon
 extern "C" int cb_embedding_gather(const long long* ids, const float* table, float* out, int n, int D, int V,
                                    void* stream) {
     CB_REQUIRE(n > 0 && D > 0 && D % 4 == 0 && V > 0, CB_ERR_ARG, "embedding_gather: bad shape");
+    CB_REQUIRE(((reinterpret_cast<uintptr_t>(table) | reinterpret_cast<uintptr_t>(out)) & 15) == 0, CB_ERR_ALIGN,
+               "embedding_gather: table and out must be 16-byte aligned");
 CB_LAUNCH((embedding_gather_kernel), n, 192, 0, reinterpret_cast<cudaStream_t>(stream), ids, table, out, n, D, V);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
@@ -447,12 +449,10 @@ extern "C" int cb_embed_inject_bwd(const float* dout, const int* map, float* dz,
 extern "C" int cb_adamw_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1,
                              float beta2, float eps, float weight_decay, int step, int* step_dev, void* stream) {
     CB_REQUIRE(n > 0 && (step >= 1 || step_dev != nullptr), CB_ERR_ARG, "adamw: bad args");
-    const float bc1 = 1.f - powf(beta1, (float)(step >= 1 ? step : 1));
-    const float bc2s = sqrtf(1.f - powf(beta2, (float)(step >= 1 ? step : 1)));
     long long blocks = (n + 255) / 256;
     if (blocks > 1184) blocks = 1184;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-CB_LAUNCH((adamw_kernel), (unsigned)blocks, 256, 0, st, p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, bc1, bc2s, step_dev);
+CB_LAUNCH((adamw_kernel), (unsigned)blocks, 256, 0, st, p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, step, step_dev);
     if (step_dev)CB_LAUNCH((bump_step_kernel), 1, 1, 0, st, step_dev);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(2);

@@ -49,6 +49,8 @@ extern "C" int cb_pack_conv_weight(const float* w, void* out, int o_dtype, int c
                                    int cin_pad, const float* out_scale, void* stream) {
     CB_REQUIRE(w && out && cout > 0 && cin > 0 && kh > 0 && kw > 0 && cout_pad >= cout && cin_pad >= cin, CB_ERR_ARG,
                "pack_conv_weight: bad args");
+    CB_REQUIRE(o_dtype == CB_F16 || o_dtype == CB_BF16 || o_dtype == CB_F32, CB_ERR_ARG,
+               "pack_conv_weight: unsupported dtype %d", o_dtype);
     const size_t total = (size_t)kh * kw * cout_pad * cin_pad;
     pack_conv_weight_kernel<<<grid_for(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         w, out, o_dtype, cout, cin, kh * kw, cout_pad, cin_pad, out_scale);
@@ -59,6 +61,8 @@ extern "C" int cb_pack_conv_weight(const float* w, void* out, int o_dtype, int c
 
 extern "C" int cb_convert_f32(const float* x, void* out, int o_dtype, long long n, float scale, void* stream) {
     CB_REQUIRE(x && out && n > 0, CB_ERR_ARG, "convert_f32: bad args");
+    CB_REQUIRE(o_dtype == CB_F16 || o_dtype == CB_BF16 || o_dtype == CB_F32, CB_ERR_ARG,
+               "convert_f32: unsupported dtype %d", o_dtype);
     convert_f32_kernel<<<grid_for((size_t)n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, out, o_dtype,
                                                                                                     (size_t)n, scale);
     CB_CUDA(cudaGetLastError());

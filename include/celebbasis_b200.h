@@ -228,6 +228,11 @@ int cb_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
  * cb_mse_fwd_bwd: ddpm.py:294-307 + :1084-1096: loss_simple[b] = mean over (C,H,W) of the squared error, and
  *   d(mean_b loss_simple[b])/dpred * gscale.
  * cb_timestep_embedding: diffusionmodules/util.py:151-171.
+ * Every dtype argument is CB_F16, CB_BF16 or CB_F32 (CB_ERR_ARG otherwise; cb_geglu_* and cb_softmax_* take the
+ * 16-bit types only); cb_act_* take CB_ACT_NONE, _SILU, _GELU or _QUICK_GELU (CB_ERR_ARG otherwise).
+ * cb_axpby2d, cb_geglu_*, cb_upsample2x_* and cb_zero_insert2x move 4 elements per access: every tensor pointer they
+ *   take must be aligned to 4 elements of its dtype (16 B for fp32, 8 B for fp16 / bf16), CB_ERR_ALIGN otherwise.
+ *   cb_geglu_* with interleave = 1 need F % 32 == 0 (whole 64-column groups), CB_ERR_ARG otherwise.
  * ------------------------------------------------------------------------------------------- */
 int cb_axpby2d(const void* x, int x_dtype, long long ldx, float a, const void* y, int y_dtype, long long ldy, float b,
                void* out, int o_dtype, long long ldo, long long rows, int cols, void* stream);
@@ -256,7 +261,8 @@ int cb_timestep_embedding(const long long* t, void* out, int o_dtype, int B, int
 
 /* ---------------------------------------------------------------------------------------------
  * Celeb-basis embedding path (fp32): the only trainable tensors of the method live here.
- * cb_embedding_gather: token_embedding(input_ids), ldm/modules/encoders/modules.py:237.
+ * cb_embedding_gather: token_embedding(input_ids), ldm/modules/encoders/modules.py:237.  table and out must be
+ *   16-byte aligned (CB_ERR_ALIGN otherwise); an id outside [0, V) takes the nearest valid row.
  * cb_celeb_mlp_fwd: EqualLinear(512->es*K, lr_mul=1)+LeakyReLU(0.2) -> 'b (e h d) -> b e h d' -> L2 normalise,
  *   ldm/modules/id_embedding/meta_net.py:27-48,61-87,266-273.  pre/coef/nrm are saved for backward.
  * cb_celeb_basis_fwd/bwd: einsum('b e h k, e k c -> b e h c', x, basis[:,1:]) + basis[:,0], meta_net.py:275-289
@@ -268,6 +274,7 @@ int cb_timestep_embedding(const long long* t, void* out, int o_dtype, int B, int
  *   bit-exact mirror of ldm/modules/id_embedding/helpers.py:6-41.
  * cb_adamw_step: torch.optim.AdamW step on the flat trainable buffer (ddpm.py:1442-1454); if step_dev is
  *   not NULL the 1-based step counter is read from (and bumped on) the device so the launch is graph-replayable.
+ *   The bias corrections are formed on the device either way: a host-counted and a device-counted run give the same bits.
  * cb_posterior_sample: DiagonalGaussianDistribution.sample * scale_factor (distributions.py:25-37, ddpm.py:590-597)
  *   with the normal draw eps supplied by the caller (the reference draws it on the CPU).
  * ------------------------------------------------------------------------------------------- */
@@ -312,7 +319,9 @@ int cb_q_sample_masked(const float* x0, const float* noise, const long long* t, 
  *   [B][H][W][3*n_chunks] face stack followed by bilinear resize to out_hw (align_corners), NHWC output with
  *   Cpad channels, image f = chunk*B + b (torch.cat(chunk(...), 0) order, meta_net.py:336-337).
  *   host_affine6 is a HOST pointer to the 6 matrix entries (trans_matrix, meta_net.py:131-142).
- * cb_channel_affine_act: eval BatchNorm2d as y = x*scale[c]+shift[c] and/or PReLU slope[c] (either may be NULL).
+ * cb_channel_affine_act: eval BatchNorm2d as y = x*scale[c]+shift[c] and/or PReLU slope[c] (the scale / shift pair or
+ *   slope may be NULL; scale and shift are given together, CB_ERR_ARG otherwise).  x and y must be aligned to 4
+ *   elements of their dtypes (CB_ERR_ALIGN otherwise); y may be x.
  * cb_l2norm_rows: F.normalize(v, dim=-1).
  * ------------------------------------------------------------------------------------------- */
 int cb_channel_affine_act(const void* x, int x_dtype, void* y, int y_dtype, const float* scale, const float* shift,
@@ -371,6 +380,7 @@ int cb_attention_bwd_dq(const void* Q, long long ldq, const void* K, long long l
  *   padded) -- the B operand of the implicit-GEMM convolution; out_scale (optional, [Cout]) folds an eval BatchNorm
  *   that follows the convolution (ldm/modules/id_embedding/iresnet.py:41-58) into the weights.
  * cb_convert_f32: out[i] = (o_dtype) (scale * x[i]) for any n.
+ * o_dtype is CB_F16, CB_BF16 or CB_F32 for both (CB_ERR_ARG otherwise).
  * ------------------------------------------------------------------------------------------- */
 int cb_pack_conv_weight(const float* w, void* out, int o_dtype, int cout, int cin, int kh, int kw, int cout_pad,
                         int cin_pad, const float* out_scale, void* stream);
