@@ -32,6 +32,7 @@ SIGS = {
     "cb_embed_inject_bwd": [_p, _p, _p, _i, _i, _i, _i, _p],
     "cb_adamw_step": [_p, _p, _p, _p, _l, _f, _f, _f, _f, _f, _i, _p, _p],
     "cb_posterior_sample": [_p, _p, _p, _i, _i, _i, _f, _p],
+    "cb_loss_mean": [_p, _p, _i, _p],
     "cb_ddim_step": [_p, _p, _p, _p, _p, _p, _l, _f, _f, _f, _f, _f, _p],
     "cb_attention_fwd": [_p, _l, _p, _l, _p, _l, _p, _l, _p, _p, _l, _i, _i, _i, _i, _i, _i, _f, _i, _p],
     "cb_attention_bwd": [_p, _l, _p, _l, _p, _l, _p, _l, _p, _l, _p, _p, _p, _l, _p, _l, _p, _l, _i, _i, _i, _i, _i, _i, _f,

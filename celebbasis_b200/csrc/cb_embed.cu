@@ -316,6 +316,15 @@ __global__ void ema_rows_kernel(float* __restrict__ table, const long long* __re
         table[(size_t)id * row + i] = v;
     }
 }
+
+// mean over the batch of the per-sample losses, summed in sample order (torch's mean of a (B,) fp32 tensor for the
+// batch sizes a training step uses): one thread, B values
+__global__ void loss_mean_kernel(const float* __restrict__ loss, float* __restrict__ out, int B) {
+    pdl_sync();
+    float s = 0.f;
+    for (int b = 0; b < B; ++b) s += loss[b];
+    out[0] = s / (float)B;
+}
 }  // namespace cb
 
 using namespace cb;
@@ -476,6 +485,14 @@ extern "C" int cb_ema_rows(float* table, const long long* idx, int idx_stride, c
     dim3 grid((unsigned)(gx < 8 ? gx : 8), (unsigned)B);
     CB_LAUNCH((ema_rows_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, idx, idx_stride, src, B, row,
               n_rows, momentum);
+    CB_CUDA(cudaGetLastError());
+    count_launches(1);
+    return 0;
+}
+
+extern "C" int cb_loss_mean(const float* loss, float* out, int B, void* stream) {
+    CB_REQUIRE(loss && out && B > 0, CB_ERR_ARG, "loss_mean: bad args");
+    CB_LAUNCH((loss_mean_kernel), 1, 1, 0, reinterpret_cast<cudaStream_t>(stream), loss, out, B);
     CB_CUDA(cudaGetLastError());
     count_launches(1);
     return 0;

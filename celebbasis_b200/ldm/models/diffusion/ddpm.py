@@ -89,18 +89,18 @@ def _plain(cfg):
 
 
 class _FusedLossFn(torch.autograd.Function):
-    """The fused step computes loss AND d(loss)/d(W, b) in one CUDA-graph replay; this node hands those gradients to
-    autograd so that the reference's `loss.backward(); optimizer.step()` contract (Lightning's loop) is unchanged."""
+    """The fused step computes loss AND d(loss)/d(trained tensors) in one CUDA-graph replay; this node hands those
+    gradients (`grads`, one per tensor of `params`) to autograd so that the reference's `loss.backward();
+    optimizer.step()` contract (Lightning's loop) is unchanged."""
 
     @staticmethod
-    def forward(ctx, W, b, loss_dev, gW, gb):
-        ctx.save_for_backward(gW, gb)
+    def forward(ctx, loss_dev, grads, *params):
+        ctx.save_for_backward(*grads)
         return loss_dev.reshape(()).clone()
 
     @staticmethod
     def backward(ctx, dloss):
-        gW, gb = ctx.saved_tensors
-        return gW * dloss, gb * dloss, None, None, None
+        return (None, None) + tuple(g * dloss for g in ctx.saved_tensors)
 
 
 class DDPM(_Base):
@@ -372,6 +372,8 @@ class LatentDiffusion(DDPM):
             return False
         if self.embedding_reg_weight > 0 or self.original_elbo_weight != 0 or self.l_simple_weight != 1.:
             return False
+        if self._textual_inversion():
+            return self._ti_fused_applicable(batch)
         io = batch.get("image_ori") if isinstance(batch, dict) else None
         x = batch.get(self.first_stage_key) if isinstance(batch, dict) else None
         if io is None or not torch.is_tensor(x) or x.dim() != 4 or x.shape[-1] != 3 or x.dtype != torch.float32:
@@ -385,7 +387,59 @@ class LatentDiffusion(DDPM):
             return False
         return next(self.model.parameters()).is_cuda
 
+    def _textual_inversion(self):
+        from ldm.modules.embedding_manager import EmbeddingManager
+        return isinstance(self.embedding_manager, EmbeddingManager)
+
+    def _ti_fused_applicable(self, batch):
+        """Textual Inversion (v1-finetune.yaml) batches: fp32 (B, H, W, 3) images with one caption each.  Progressive
+        words change the number of injected vectors with the step counter and stay on the eager path; the manager
+        rejects per_image_tokens when it is built."""
+        if self.embedding_manager.progressive_words or not isinstance(batch, dict):
+            return False
+        x, cap = batch.get(self.first_stage_key), batch.get(self.cond_stage_key)
+        if not torch.is_tensor(x) or x.dim() != 4 or x.shape[-1] != 3 or x.dtype != torch.float32:
+            return False
+        if not isinstance(cap, (list, tuple)) or len(cap) != x.shape[0] or not all(isinstance(c, str) for c in cap):
+            return False
+        return next(self.model.parameters()).is_cuda
+
+    def _ti_params(self):
+        em = self.embedding_manager
+        return [em.string_to_param_dict[k] for k in em.string_to_token_dict]
+
+    def _ti_prepare(self, eng, captions):
+        """Host side of the TI step: tokenise and build the inject map with the manager's own arithmetic (no sync)."""
+        ids = eng.tokenize(captions)
+        map_np, _ = self.embedding_manager.ti_map(ids.numpy())
+        self.embedding_manager.last_map = map_np
+        return ids, map_np
+
+    def _fused_build_ti(self, batch):
+        from celebbasis_b200.step_graph import StepGraphs
+        from celebbasis_b200.train_step import TextualInversionStep
+        x = batch[self.first_stage_key]
+        B, hw = x.shape[0], x.shape[1]
+        params = self._ti_params()
+        dev = params[0].device
+        eng = TextualInversionStep(self._engine_params, self.state_dict(), [p.detach() for p in params], dev,
+                                   tokenizer=self.cond_stage_model.tokenizer, lr=self.learning_rate)
+        # the placeholder parameters alias the engine's flat buffer: FusedAdamW, save() and the graphs see one memory
+        for p, view in zip(params, eng.params):
+            p.data = view
+        T = getattr(self.cond_stage_model, "max_length", 77)
+        G = StepGraphs(eng, B=B, T=T, n_chunks=0, image_hw=hw)
+        ids, map_np = self._ti_prepare(eng, batch[self.cond_stage_key])
+        lat = G.noise.shape[-1]
+        G.load_next(x, None, torch.zeros(B, 4, lat, lat))
+        G.load_step(ids, map_np, torch.zeros(B, dtype=torch.long), torch.zeros_like(G.noise))
+        G.capture()
+        self._fused, self._fused_sig = G, (B, hw, 0, dev)
+        return G
+
     def _fused_build(self, batch):
+        if self._textual_inversion():
+            return self._fused_build_ti(batch)
         from celebbasis_b200.step_graph import StepGraphs
         from celebbasis_b200.train_step import CelebBasisStep
         x = batch[self.first_stage_key]
@@ -416,32 +470,39 @@ class LatentDiffusion(DDPM):
         return G
 
     def _fused_shared_step(self, batch):
+        ti = self._textual_inversion()
+        faces_of = (lambda b: None) if ti else (lambda b: b["image_ori"]["faces"])
         x = batch[self.first_stage_key]
-        io = batch["image_ori"]
         B, hw = x.shape[0], x.shape[1]
         G = self._fused
         dev = next(self.model.parameters()).device
-        if G is None or self._fused_sig != (B, hw, io["faces"].shape[-1] // 3, dev):
+        if G is None or self._fused_sig != (B, hw, 0 if ti else faces_of(batch).shape[-1] // 3, dev):
             G = self._fused_build(batch)
         eng = G.eng
         lat_shape = list(G.peps_n.shape)
         if G.next_token is not batch:                         # no look-ahead happened for this batch: front end now
-            G.load_next(x, io["faces"], torch.randn(lat_shape))       # posterior eps from the CPU generator, as
+            G.load_next(x, faces_of(batch), torch.randn(lat_shape))   # posterior eps from the CPU generator, as
             G.prefetch(batch)                                          # distributions.py:36 does
-        ids, map_np, positions = eng.prepare(batch["caption"])        # tokenise + bit-exact placeholder row map (host)
-        self.embedding_manager.last_positions = positions
+        if ti:
+            ids, map_np = self._ti_prepare(eng, batch[self.cond_stage_key])
+        else:
+            ids, map_np, positions = eng.prepare(batch["caption"])    # tokenise + bit-exact placeholder row map (host)
+            self.embedding_manager.last_positions = positions
         t = torch.randint(0, self.num_timesteps, (B,), device=dev).long()
         noise = torch.randn_like(G.z)
-        G.load_step(ids, map_np, t, noise, io["ids"])
+        G.load_step(ids, map_np, t, noise, None if ti else batch["image_ori"]["ids"])
         nxt, self._staged_next = self._staged_next, None
         if nxt is not None and (nxt is batch or not self._fused_applicable(nxt)
                                 or nxt[self.first_stage_key].shape != x.shape):
             nxt = None
         if nxt is not None:
-            G.load_next(nxt[self.first_stage_key], nxt["image_ori"]["faces"], torch.randn(lat_shape))
+            G.load_next(nxt[self.first_stage_key], faces_of(nxt), torch.randn(lat_shape))
         loss_dev = G.step(lookahead=nxt is not None, token=nxt)
-        lin = self.embedding_manager.meta_id_net.stylegan_mlp.net[0]
-        loss = _FusedLossFn.apply(lin.weight, lin.bias, loss_dev, eng.gW, eng.gb)
+        if ti:
+            loss = _FusedLossFn.apply(loss_dev, eng.grads, *self._ti_params())
+        else:
+            lin = self.embedding_manager.meta_id_net.stylegan_mlp.net[0]
+            loss = _FusedLossFn.apply(loss_dev, (eng.gW, eng.gb), lin.weight, lin.bias)
         loss_simple = eng.last["loss_simple"].detach()
         prefix = 'train' if self.training else 'val'
         loss_dict = {f'{prefix}/loss_simple': loss_simple.mean(),

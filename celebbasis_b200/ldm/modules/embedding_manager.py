@@ -279,11 +279,11 @@ class EmbeddingManager(nn.Module):
         self._zero_pos = None
         self.last_map = None
 
-    def forward(self, tokenized_text, embedded_text, face_image=None, img_ori=None, celeb_embeddings=None):
-        b, n = tokenized_text.shape
-        device = embedded_text.device
-        placeholders, z_list, base = [], [], 0
-        steps = []
+    def ti_map(self, tok_host):
+        """The inject map of (B, n) host token ids: (map (B, n) int32 over the original rows / -(z row + 1), rewritten
+        token ids).  z rows are the placeholders' parameters concatenated in the dict's order."""
+        b, n = tok_host.shape
+        placeholders, base, steps = [], 0, []
         for key, ptoken in self.string_to_token_dict.items():
             p = self.string_to_param_dict[key]
             if self.max_vectors_per_token > 1 and self.progressive_words:
@@ -292,9 +292,7 @@ class EmbeddingManager(nn.Module):
             else:
                 steps.append(self.max_vectors_per_token)
             placeholders.append((int(ptoken), base, p.shape[0]))
-            z_list.append(p.to(device))
             base += p.shape[0]
-        tok_host = tokenized_text.detach().cpu().numpy()
         # per-placeholder active length: apply them one at a time so each sees its own max_step_tokens
         cur_tok = tok_host
         maps = np.tile(np.arange(n, dtype=np.int32), (b, 1))
@@ -304,11 +302,17 @@ class EmbeddingManager(nn.Module):
             sel = m >= 0
             new = np.where(sel, np.take_along_axis(maps, np.clip(m, 0, n - 1), axis=1), m)
             maps = new.astype(np.int32)
+        return maps, cur_tok
+
+    def forward(self, tokenized_text, embedded_text, face_image=None, img_ori=None, celeb_embeddings=None):
+        b, n = tokenized_text.shape
+        device = embedded_text.device
+        maps, cur_tok = self.ti_map(tokenized_text.detach().cpu().numpy())
         if self.max_vectors_per_token > 1:
             tokenized_text.copy_(torch.from_numpy(cur_tok).to(tokenized_text.device))     # in-place, like the reference
         self.last_map = maps
         map_dev = torch.from_numpy(maps).to(device)
-        z_rows = torch.cat(z_list, 0).float()
+        z_rows = torch.cat([self.string_to_param_dict[k].to(device) for k in self.string_to_token_dict], 0).float()
         if self._zero_pos is None or self._zero_pos.device != device or self._zero_pos.shape[0] < n:
             self._zero_pos = torch.zeros(n, embedded_text.shape[-1], dtype=torch.float32, device=device)
         return _InjectFn.apply(embedded_text, z_rows, map_dev, self._zero_pos)

@@ -737,9 +737,11 @@ def embed_inject_fwd(tok, z_rows, map_, pos, B, T):
     return out
 
 
-def embed_inject_bwd(dout, map_, n_z_rows, B, T):
+def embed_inject_bwd(dout, map_, n_z_rows, B, T, out=None):
+    """Gradient of the z rows (every row written; a row no prompt uses gets 0); `out` may be a (n_z_rows, D) view."""
     D = dout.shape[1]
-    dz = torch.empty(n_z_rows, D, dtype=torch.float32, device=dout.device)
+    dz = torch.empty(n_z_rows, D, dtype=torch.float32, device=dout.device) if out is None else out
+    assert dz.shape == (n_z_rows, D) and dz.is_contiguous()
     _lib.check(_L().cb_embed_inject_bwd(_p(dout), _p(map_), _p(dz), n_z_rows, B, T, D, _st()), "cb_embed_inject_bwd")
     return dz
 
@@ -747,6 +749,13 @@ def embed_inject_bwd(dout, map_, n_z_rows, B, T):
 def adamw_step(p, g, m, v, *, lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=1e-2, step=0, step_dev=None):
     _lib.check(_L().cb_adamw_step(_p(p), _p(g), _p(m), _p(v), p.numel(), lr, beta1, beta2, eps, weight_decay, step,
                                   _p(step_dev), _st()), "cb_adamw_step")
+
+
+def loss_mean(loss):
+    """(B,) per-sample losses -> (1,) batch mean (cb_loss_mean)."""
+    out = torch.empty(1, dtype=torch.float32, device=loss.device)
+    _lib.check(_L().cb_loss_mean(_p(loss), _p(out), loss.shape[0], _st()), "cb_loss_mean")
+    return out
 
 
 def posterior_sample(moments_nchw, eps, scale):

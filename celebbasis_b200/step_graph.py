@@ -7,6 +7,9 @@ WHILE batch i trains: its throughput-bound 512^2 convolutions fill the SMs that 
 CLIP launches leaves idle.  Every step still does all of its work exactly once (K steps = K front ends + K chains); the
 pipeline only changes when the front end of a batch is executed.
 
+The same executor runs the Textual Inversion step (train_step.TextualInversionStep, n_chunks=0): its front end is the
+VAE encode alone, and no face buffers exist.
+
 Three graphs over static buffers (torch is buffers / streams / graph capture only):
 
   G_pre   front end of the batch in the `next` input slot -> (z_next, v_next)
@@ -29,20 +32,21 @@ class StepGraphs:
         self.B, self.T, self.n_chunks = B, T, n_chunks
         lat = image_hw // 8
         f32 = dict(dtype=torch.float32, device=dev)
+        faces = n_chunks > 0        # n_chunks = 0: a step without face crops (Textual Inversion)
         # `next` slot: raw inputs of the batch whose front end runs next
         self.image_n = torch.zeros(B, image_hw, image_hw, 3, **f32)
-        self.faces_n = torch.zeros(B, image_hw, image_hw, 3 * n_chunks, **f32)
+        self.faces_n = torch.zeros(B, image_hw, image_hw, 3 * n_chunks, **f32) if faces else None
         self.peps_n = torch.zeros(B, 4, lat, lat, **f32)
         self.z_n = torch.zeros(B, 4, lat, lat, **f32)
-        self.v_n = torch.zeros(n_chunks * B, 512, **f32)
+        self.v_n = torch.zeros(n_chunks * B, 512, **f32) if faces else None
         # `cur` slot: what the chain consumes
         self.z = torch.zeros(B, 4, lat, lat, **f32)
-        self.v = torch.zeros(n_chunks * B, 512, **f32)
+        self.v = torch.zeros(n_chunks * B, 512, **f32) if faces else None
         self.ids = torch.zeros(B, T, dtype=torch.int64, device=dev)
         self.map = torch.zeros(B, T, dtype=torch.int32, device=dev)
         self.t = torch.zeros(B, dtype=torch.int64, device=dev)
         self.noise = torch.zeros(B, 4, lat, lat, **f32)
-        self.ids_person = torch.zeros(B, n_chunks, dtype=torch.int64, device=dev)
+        self.ids_person = torch.zeros(B, n_chunks, dtype=torch.int64, device=dev) if faces else None
         self.loss = None
         self.outs = {}              # per graph: (loss tensor, eng.last of that capture) -- static addresses per graph
         self.use_graphs = graphs
@@ -53,15 +57,17 @@ class StepGraphs:
     # ---- input staging (host or device sources; pinned host memory makes the copies asynchronous) -----------------
     def load_next(self, image, faces, posterior_eps):
         self.image_n.copy_(image, non_blocking=True)
-        self.faces_n.copy_(faces, non_blocking=True)
+        if self.faces_n is not None:
+            self.faces_n.copy_(faces, non_blocking=True)
         self.peps_n.copy_(posterior_eps, non_blocking=True)
 
-    def load_step(self, ids, map_, t, noise, ids_person):
+    def load_step(self, ids, map_, t, noise, ids_person=None):
         self.ids.copy_(ids, non_blocking=True)
         self.map.copy_(map_ if torch.is_tensor(map_) else torch.from_numpy(map_), non_blocking=True)
         self.t.copy_(t, non_blocking=True)
         self.noise.copy_(noise, non_blocking=True)
-        self.ids_person.copy_(ids_person, non_blocking=True)
+        if self.ids_person is not None:
+            self.ids_person.copy_(ids_person, non_blocking=True)
 
     # ---- the three bodies ------------------------------------------------------------------------------------------
     def _front_end(self):
@@ -69,7 +75,8 @@ class StepGraphs:
 
     def _promote(self):
         self.z.copy_(self.z_n)
-        self.v.copy_(self.v_n)
+        if self.v is not None:
+            self.v.copy_(self.v_n)
 
     def _chain(self):
         self.loss = self.eng.stage_main(self.z, self.v, self.ids_person, self.ids, self.map, self.t, self.noise)
@@ -113,7 +120,7 @@ class StepGraphs:
         from . import lib
         eng = self.eng
         eng._warm = True
-        coef0, emb0 = eng.id_coefficients.clone(), eng.id_embeddings.clone()    # the warm-up steps move the EMA state
+        state0 = [x.clone() for x in eng.ema_state()]       # the warm-up steps move the EMA state
         for _ in range(2):
             self._body_pre()
             self._body_main()
@@ -139,8 +146,8 @@ class StepGraphs:
             if name != "pre":
                 self.outs[name] = (self.loss, self._last)
         torch.cuda.synchronize()
-        eng.id_coefficients.copy_(coef0)
-        eng.id_embeddings.copy_(emb0)
+        for x, x0 in zip(eng.ema_state(), state0):
+            x.copy_(x0)
         return self
 
     def _run(self, name):

@@ -82,10 +82,14 @@ def build_inject_map(ids, placeholder_token, reps, z_row_of_sample):
     return build_inject_map_multi(ids, [([placeholder_token], [z_row_of_sample(b) * reps]) for b in range(B)], reps)
 
 
-class CelebBasisStep:
-    def __init__(self, params, state_dict, basis, device, *, tokenizer, placeholder="sks", clip_layers=None,
-                 dtype=torch.float16, loss_scale=1024.0, vae_res_dtype=torch.float32, lr=5e-3, id_coefficients=None,
-                 id_embeddings=None):
+class _LatentTrainStep:
+    """What both training steps share: the frozen UNet / CLIP text / VAE encoder engines, the noise schedule, the front
+    end (VAE encode + posterior sample) and the trainable chain's tail (token gather -> inject of the trained rows -> CLIP
+    text -> UNet -> MSE -> UNet / CLIP backward -> gradient of the rows).  A subclass says where the injected rows come
+    from (_rows_fwd) and where their gradient goes (_rows_bwd)."""
+
+    def __init__(self, params, state_dict, device, *, tokenizer, dtype=torch.float16, loss_scale=1024.0,
+                 vae_res_dtype=torch.float32, lr=5e-3):
         self.dev = torch.device(device)
         self.dt = dtype
         sd = state_dict
@@ -96,31 +100,11 @@ class CelebBasisStep:
         fs = params["first_stage_config"]["params"]
         self.vae = VAEEncoderEngine(fs["ddconfig"], fs["embed_dim"], sub("first_stage_model."), self.dev, dtype=dtype,
                                     res_dtype=vae_res_dtype)
-        self.face = IResNetEngine(sub("embedding_manager.meta_id_net.id_model."), self.dev, dtype=dtype)
-        pc = params["personalization_config"]["params"]
-        self.es = pc["num_embeds_per_token"]
-        self.K = pc["meta_inner_dim"]
-        self.momentum = pc.get("momentum", 0.9)
-        self.max_ids = pc.get("max_ids", 10)
-        self.W = sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.weight"].detach().to(self.dev, torch.float32).contiguous()
-        self.b = sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.bias"].detach().to(self.dev, torch.float32).contiguous()
-        # trainable tensors live in ONE flat fp32 buffer (what the data-parallel all-reduce and AdamW operate on)
-        self.flat = torch.cat([self.W.flatten(), self.b.flatten()]).contiguous()
-        self.W = self.flat[: self.W.numel()].view_as(self.W)
-        self.b = self.flat[self.W.numel():]
-        self.grad = torch.zeros_like(self.flat)
-        self.gW = self.grad[: self.W.numel()].view_as(self.W)
-        self.gb = self.grad[self.W.numel():]
-        self.adam_m = torch.zeros_like(self.flat)
-        self.adam_v = torch.zeros_like(self.flat)
         self.step_dev = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.lr = lr
-        self.overlap_branches = True     # VAE encode || face net + CLIP text on two streams (see run())
         self._side = None
         self._warm = False
-        self.basis = basis.detach().to(self.dev, torch.float32).contiguous()
         self.tokenizer = tokenizer
-        self.placeholder_token = int(tokenizer(placeholder)["input_ids"][0, 1])
         self.scale_factor = float(params["scale_factor"])
         # schedule (ddpm.py:126-178; util.py:21-25: float64 linspace of sqrt(beta), squared)
         T = params["timesteps"]
@@ -129,6 +113,123 @@ class CelebBasisStep:
         self.sqrt_ac = torch.tensor(np.sqrt(ac), dtype=torch.float32, device=self.dev)
         self.sqrt_1mac = torch.tensor(np.sqrt(1.0 - ac), dtype=torch.float32, device=self.dev)
         self.num_timesteps = T
+        self._prio = None
+        self.last = {}
+
+    def _init_flat(self, tensors):
+        """The trainable tensors live in ONE flat fp32 buffer (what the data-parallel all-reduce and AdamW operate on);
+        returns views of it and of the gradient buffer shaped like `tensors`."""
+        self.flat = torch.cat([t.detach().to(self.dev, torch.float32).reshape(-1) for t in tensors]).contiguous()
+        self.grad = torch.zeros_like(self.flat)
+        self.adam_m = torch.zeros_like(self.flat)
+        self.adam_v = torch.zeros_like(self.flat)
+        views, grads, off = [], [], 0
+        for t in tensors:
+            views.append(self.flat[off: off + t.numel()].view(t.shape))
+            grads.append(self.grad[off: off + t.numel()].view(t.shape))
+            off += t.numel()
+        return views, grads
+
+    def tokenize(self, captions):
+        return self.tokenizer(captions, truncation=True, max_length=77, return_length=True,
+                              return_overflowing_tokens=False, padding="max_length", return_tensors="pt")["input_ids"]
+
+    def encode_first_stage(self, image_nhwc, posterior_eps):
+        """get_input (ddpm.py:344-350,702-759): HWC->CHW, VAE encode, posterior sample * scale_factor."""
+        x = image_nhwc.permute(0, 3, 1, 2).contiguous().float()   # layout glue exactly as ddpm.py:348-349
+        moments = self.vae.encode_moments(x)
+        z = ops.posterior_sample(moments, posterior_eps.contiguous(), self.scale_factor)
+        return z, moments
+
+    def q_sample(self, z, t, noise):
+        """ddpm.py:289-292 per sample (the two coefficients are device scalars gathered by t)."""
+        return ops.q_sample(z.contiguous(), noise.contiguous(), t.contiguous(), self.sqrt_ac, self.sqrt_1mac)
+
+    def _side_stream(self):
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.dev)
+        return self._side
+
+    def _aux_stream(self):
+        if getattr(self, "_aux", None) is None:
+            self._aux = torch.cuda.Stream(device=self.dev, priority=-1)
+        return self._aux
+
+    def _prio_stream(self):
+        if self._prio is None:
+            self._prio = torch.cuda.Stream(device=self.dev, priority=-1)
+        return self._prio
+
+    def ema_state(self):
+        """Device tensors a step updates besides the gradient (restored after StepGraphs' warm-up steps)."""
+        return ()
+
+    def stage_main(self, z, v, ids_person, ids_dev, map_dev, t, noise, *, need_grad=True, ema_update=True):
+        """Everything downstream of the frozen front end: the rows to inject -> inject -> CLIP text -> UNet -> loss ->
+        backward to the trained tensors.  Returns the loss; gradients land in self.grad."""
+        B, T = z.shape[0], ids_dev.shape[1]
+        # the text branch (rows -> inject -> 12 CLIP layers, ~110 small launches) runs beside the UNet's prefix (timestep
+        # MLP, stem, first ResBlock, first self-attention): the UNet waits for the context at its first cross-attention
+        main = torch.cuda.current_stream()
+        aux = self._aux_stream()
+        fork = torch.cuda.Event()
+        fork.record(main)
+        aux.wait_event(fork)
+        with torch.cuda.stream(aux), ops.lane(3):
+            rows, saved = self._rows_fwd(v)
+            tok = ops.embedding_gather(ids_dev.view(-1), self.clip.tok_table)
+            emb = ops.embed_inject_fwd(tok, rows, map_dev.view(-1), self.clip.pos_table, B, T)
+            context = self.clip.forward(emb, B, need_grad=need_grad)
+            ctx_ready = torch.cuda.Event()
+            ctx_ready.record(aux)
+        noise = noise.contiguous()
+        x_noisy = self.q_sample(z, t, noise)
+        eps = self.unet.forward(x_noisy, t, context.view(B, T, -1), need_grad=need_grad, context_ready=ctx_ready)
+        main.wait_event(ctx_ready)      # (already implied by the UNet's first cross-attention; explicit for the EMA / backward)
+        loss_simple, d_eps = ops.mse_fwd_bwd(eps, noise, 1.0, want_grad=need_grad)
+        loss = loss_simple if B == 1 else ops.loss_mean(loss_simple)
+        self.last = dict(z=z, context=context.view(B, T, -1), eps=eps, x_noisy=x_noisy, loss_simple=loss_simple,
+                         **self._rows_last(saved, v))
+        if ema_update:
+            self._rows_ema(saved, ids_person, B)
+        if need_grad:
+            dctx = self.unet.backward(d_eps)
+            demb = self.clip.backward(dctx.view(B * T, -1))
+            self._rows_bwd(demb, map_dev, B, T, saved, v)
+        return loss
+
+    def _rows_last(self, saved, v):
+        return {}
+
+    def _rows_ema(self, saved, ids_person, B):
+        pass
+
+    def optimizer_step(self, lr=None):
+        """torch.optim.AdamW defaults (ddpm.py:1442-1454): betas (.9,.999), eps 1e-8, weight_decay 1e-2."""
+        ops.adamw_step(self.flat, self.grad, self.adam_m, self.adam_v, lr=self.lr if lr is None else lr,
+                       step_dev=self.step_dev)
+
+
+class CelebBasisStep(_LatentTrainStep):
+    def __init__(self, params, state_dict, basis, device, *, tokenizer, placeholder="sks", clip_layers=None,
+                 dtype=torch.float16, loss_scale=1024.0, vae_res_dtype=torch.float32, lr=5e-3, id_coefficients=None,
+                 id_embeddings=None):
+        super().__init__(params, state_dict, device, tokenizer=tokenizer, dtype=dtype, loss_scale=loss_scale,
+                         vae_res_dtype=vae_res_dtype, lr=lr)
+        sd = state_dict
+        sub = lambda pre: {k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}
+        self.face = IResNetEngine(sub("embedding_manager.meta_id_net.id_model."), self.dev, dtype=dtype)
+        self.overlap_branches = True     # VAE encode || face net + CLIP text on two streams (see run())
+        pc = params["personalization_config"]["params"]
+        self.es = pc["num_embeds_per_token"]
+        self.K = pc["meta_inner_dim"]
+        self.momentum = pc.get("momentum", 0.9)
+        self.max_ids = pc.get("max_ids", 10)
+        (self.W, self.b), (self.gW, self.gb) = self._init_flat(
+            [sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.weight"],
+             sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.bias"]])
+        self.basis = basis.detach().to(self.dev, torch.float32).contiguous()
+        self.placeholder_token = int(tokenizer(placeholder)["input_ids"][0, 1])
         # per-identity EMA side state, initialised as EmbeddingManagerId does (embedding_manager.py:229-252): ONE randn
         # coefficient tensor shared by every identity, embeddings = the initializer word's token embedding
         self.test_mode = pc.get("test_mode", "coefficient")
@@ -147,29 +248,11 @@ class CelebBasisStep:
             .to(self.dev).contiguous()
         self.id_embeddings = torch.stack([e.detach().float().reshape(self.es, -1) for e in id_embeddings]) \
             .to(self.dev).contiguous()
-        self._prio = None
-        self.last = {}
-
-    # ------------------------------------------------------------------------------------------
-    def tokenize(self, captions):
-        return self.tokenizer(captions, truncation=True, max_length=77, return_length=True,
-                              return_overflowing_tokens=False, padding="max_length", return_tensors="pt")["input_ids"]
-
-    def encode_first_stage(self, image_nhwc, posterior_eps):
-        """get_input (ddpm.py:344-350,702-759): HWC->CHW, VAE encode, posterior sample * scale_factor."""
-        x = image_nhwc.permute(0, 3, 1, 2).contiguous().float()   # layout glue exactly as ddpm.py:348-349
-        moments = self.vae.encode_moments(x)
-        z = ops.posterior_sample(moments, posterior_eps.contiguous(), self.scale_factor)
-        return z, moments
 
     def face_features(self, faces, n_chunks):
         x, geo = ops.face_warp_resize(faces.contiguous(), n_chunks, TRANS_MATRIX, out_hw=112, cpad=8, dtype=self.dt)
         feat = self.face.forward(x, geo)
         return ops.l2norm_rows(feat)
-
-    def q_sample(self, z, t, noise):
-        """ddpm.py:289-292 per sample (the two coefficients are device scalars gathered by t)."""
-        return ops.q_sample(z.contiguous(), noise.contiguous(), t.contiguous(), self.sqrt_ac, self.sqrt_1mac)
 
     # ------------------------------------------------------------------------------------------
     def prepare(self, captions):
@@ -240,11 +323,6 @@ class CelebBasisStep:
             self.last.update(d_eps=d_eps, dctx=dctx, demb=demb, dz=dz, dcoef=dcoef)
         return loss
 
-    def _side_stream(self):
-        if self._side is None:
-            self._side = torch.cuda.Stream(device=self.dev)
-        return self._side
-
     def _ema_update(self, zc, coef, ids_person, B):
         """_momentum_update, training branch (embedding_manager.py:484-489) for the main identity of each sample; the
         identity index is read on the device (no host sync, CUDA-graph safe)."""
@@ -278,53 +356,26 @@ class CelebBasisStep:
         main.wait_event(join)
         return (z if z_out is None else z_out), (v if v_out is None else v_out)
 
-    def stage_main(self, z, v, ids_person, ids_dev, map_dev, t, noise, *, need_grad=True, ema_update=True):
-        """Everything downstream of the trainable MLP: celeb-basis embeddings -> inject -> CLIP text -> UNet -> loss ->
-        backward to (W, b).  Returns the loss; gradients land in self.grad."""
-        B, T = z.shape[0], ids_dev.shape[1]
-        # the text branch (MLP -> basis -> inject -> 12 CLIP layers, ~110 small launches) runs beside the UNet's prefix
-        # (timestep MLP, stem, first ResBlock, first self-attention): the UNet waits for the context at its first
-        # cross-attention
-        main = torch.cuda.current_stream()
-        aux = self._aux_stream()
-        fork = torch.cuda.Event()
-        fork.record(main)
-        aux.wait_event(fork)
-        with torch.cuda.stream(aux), ops.lane(3):
-            pre, coef, nrm = ops.celeb_mlp_fwd(v, self.W, self.b, self.es)
-            zc = ops.celeb_basis_fwd(coef, self.basis)
-            tok = ops.embedding_gather(ids_dev.view(-1), self.clip.tok_table)
-            emb = ops.embed_inject_fwd(tok, zc.view(-1, zc.shape[-1]), map_dev.view(-1), self.clip.pos_table, B, T)
-            context = self.clip.forward(emb, B, need_grad=need_grad)
-            ctx_ready = torch.cuda.Event()
-            ctx_ready.record(aux)
-        noise = noise.contiguous()
-        x_noisy = self.q_sample(z, t, noise)
-        eps = self.unet.forward(x_noisy, t, context.view(B, T, -1), need_grad=need_grad, context_ready=ctx_ready)
-        main.wait_event(ctx_ready)      # (already implied by the UNet's first cross-attention; explicit for the EMA / backward)
-        loss_simple, d_eps = ops.mse_fwd_bwd(eps, noise, 1.0, want_grad=need_grad)
-        loss = loss_simple if B == 1 else loss_simple.mean(0, keepdim=True)
-        self.last = dict(z=z, context=context.view(B, T, -1), eps=eps, x_noisy=x_noisy, coef=coef, celeb_z=zc,
-                         face_feat=v, loss_simple=loss_simple)
-        if ema_update:
-            self._ema_update(zc, coef, ids_person, B)
-        if need_grad:
-            dctx = self.unet.backward(d_eps)
-            demb = self.clip.backward(dctx.view(B * T, -1))
-            dz = ops.embed_inject_bwd(demb, map_dev.view(-1), zc.shape[0] * self.es, B, T)
-            dcoef = ops.celeb_basis_bwd(dz.view(zc.shape), self.basis)
-            ops.celeb_mlp_bwd(dcoef, coef, nrm, pre, v, self.gW, self.gb)
-        return loss
+    # the trainable part of the chain (_LatentTrainStep.stage_main): celeb-basis MLP -> basis -> 2 rows per face
+    def _rows_fwd(self, v):
+        pre, coef, nrm = ops.celeb_mlp_fwd(v, self.W, self.b, self.es)
+        zc = ops.celeb_basis_fwd(coef, self.basis)
+        return zc.view(-1, zc.shape[-1]), (pre, coef, nrm, zc)
 
-    def _aux_stream(self):
-        if getattr(self, "_aux", None) is None:
-            self._aux = torch.cuda.Stream(device=self.dev, priority=-1)
-        return self._aux
+    def _rows_last(self, saved, v):
+        return dict(coef=saved[1], celeb_z=saved[3], face_feat=v)
 
-    def _prio_stream(self):
-        if self._prio is None:
-            self._prio = torch.cuda.Stream(device=self.dev, priority=-1)
-        return self._prio
+    def _rows_ema(self, saved, ids_person, B):
+        self._ema_update(saved[3], saved[1], ids_person, B)
+
+    def _rows_bwd(self, demb, map_dev, B, T, saved, v):
+        pre, coef, nrm, zc = saved
+        dz = ops.embed_inject_bwd(demb, map_dev.view(-1), zc.shape[0] * self.es, B, T)
+        dcoef = ops.celeb_basis_bwd(dz.view(zc.shape), self.basis)
+        ops.celeb_mlp_bwd(dcoef, coef, nrm, pre, v, self.gW, self.gb)
+
+    def ema_state(self):
+        return (self.id_coefficients, self.id_embeddings)
 
     # ---- checkpoint (embedding_manager.py:396-410): the file stable_txt2img.py:230 loads -----------------------
     def gathered_identity_state(self, owned_ids=None):
@@ -354,7 +405,37 @@ class CelebBasisStep:
             torch.save(out, path)
         return out
 
-    def optimizer_step(self, lr=None):
-        """torch.optim.AdamW defaults (ddpm.py:1442-1454): betas (.9,.999), eps 1e-8, weight_decay 1e-2."""
-        ops.adamw_step(self.flat, self.grad, self.adam_m, self.adam_v, lr=self.lr if lr is None else lr,
-                       step_dev=self.step_dev)
+
+class TextualInversionStep(_LatentTrainStep):
+    """One Textual Inversion training step (configs/stable-diffusion/v1-finetune.yaml: EmbeddingManager,
+    ldm/modules/embedding_manager.py:38-184) on the sm_90a kernels:
+
+        image --VAE encode--> z --q_sample(t, noise)--> x_t ----------------------------------------\
+        caption --tokenise--> ids --gather--> token rows --inject the placeholders' rows @map--> +pos --> CLIP text --> UNet
+        loss = MSE(eps, noise);  backward: UNet -> d(context) -> CLIP -> d(embeddings) -> d(rows) (summed over occurrences)
+
+    The trained rows of every placeholder (num_vectors_per_token x 768 each, in the manager's dict order) are one flat
+    fp32 buffer; `rows` holds them in that order as the (R, 768) z table of the inject kernel.  The row map comes from the
+    manager's own host arithmetic (EmbeddingManager.ti_map), so the fused and the eager step inject the same rows."""
+
+    def __init__(self, params, state_dict, placeholder_params, device, *, tokenizer, dtype=torch.float16,
+                 loss_scale=1024.0, vae_res_dtype=torch.float32, lr=5e-3):
+        super().__init__(params, state_dict, device, tokenizer=tokenizer, dtype=dtype, loss_scale=loss_scale,
+                         vae_res_dtype=vae_res_dtype, lr=lr)
+        self.params, self.grads = self._init_flat(list(placeholder_params))
+        self.rows = self.flat.view(-1, self.clip.hidden)
+        self.grad_rows = self.grad.view(-1, self.clip.hidden)
+
+    def stage_prefetch(self, image, faces, n_chunks, posterior_eps, z_out=None, v_out=None):
+        """get_input's VAE encode + posterior sample (ddpm.py:702-759); there are no face crops."""
+        with ops.lane(2):
+            z, _ = self.encode_first_stage(image, posterior_eps)
+            if z_out is not None:
+                z_out.copy_(z)
+        return (z if z_out is None else z_out), None
+
+    def _rows_fwd(self, v):
+        return self.rows, None
+
+    def _rows_bwd(self, demb, map_dev, B, T, saved, v):
+        ops.embed_inject_bwd(demb, map_dev.view(-1), self.rows.shape[0], B, T, out=self.grad_rows)

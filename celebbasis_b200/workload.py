@@ -67,6 +67,41 @@ def synth_batch(kind="full", B=1, seed=1234, step=0):
     return batch, draws
 
 
+def ti_model_params(kind="full", num_vectors_per_token=2):
+    """configs/stable-diffusion/v1-finetune.yaml:model.params (Textual Inversion: EmbeddingManager, placeholder '*',
+    initializer word 'person') on the same UNet / VAE / CLIP sizes as model_params(kind)."""
+    p = model_params(kind)
+    p["personalization_config"] = dict(
+        target="ldm.modules.embedding_manager.EmbeddingManager",
+        params=dict(placeholder_strings=["*"], initializer_words=["person"], per_image_tokens=False,
+                    num_vectors_per_token=num_vectors_per_token, progressive_words=False))
+    return p
+
+
+def synth_photo_files(out_dir, seed=0, sizes=((40, 56), (64, 48), (37, 37), (50, 33)), modes=("RGB", "RGBA", "L", "P")):
+    """Seeded synthetic photos for PersonalizedBase: lossless PNGs, non-square, one per PIL mode (a smooth colour field
+    plus noise, so every resampling filter gives different pixels).  Returns the written paths."""
+    import os
+    import numpy as np
+    from PIL import Image
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.RandomState(seed)
+    paths = []
+    for i, ((h, w), mode) in enumerate(zip(sizes, modes)):
+        low = rng.rand(6, 6, 3)
+        img = np.asarray(Image.fromarray((low * 255).astype(np.uint8)).resize((w, h), Image.BICUBIC), dtype=np.float32)
+        img = Image.fromarray(np.clip(img + rng.randn(h, w, 3) * 12.0, 0, 255).astype(np.uint8))
+        if mode == "RGBA":
+            img = img.convert("RGBA")
+            img.putalpha(Image.fromarray(rng.randint(0, 256, (h, w)).astype(np.uint8)))
+        elif mode != "RGB":
+            img = img.convert(mode)
+        p = os.path.join(out_dir, f"photo_{i}.png")
+        img.save(p)
+        paths.append(p)
+    return paths
+
+
 def synth_face_files(out_dir, n=4, hw=64, seed=0):
     """n deterministic smooth colour images (stand-ins for aligned face crops) written as lossless PNGs named like the
     reference's fixtures (`0000N_idN.png`: identity = file stem) + the pickle FaceIdDataset* reads (gen_pickle.py: a list

@@ -294,6 +294,9 @@ int cb_adamw_step(float* p, const float* g, float* m, float* v, long long n, flo
                   float eps, float weight_decay, int step, int* step_dev, void* stream);
 int cb_posterior_sample(const float* moments, const float* eps, float* z, int N, int Cz, int HW, float scale,
                         void* stream);
+/* cb_loss_mean: out[0] = (loss[0] + ... + loss[B-1]) / B, added in sample order: the batch mean of the per-sample
+ *   losses (ddpm.py:1084-1096) inside a captured training step. */
+int cb_loss_mean(const float* loss, float* out, int B, void* stream);
 /* cb_ddim_step: one DDIM update with classifier-free guidance, ldm/models/diffusion/ddim.py:166-204:
  *   e = e_u + s*(e_c - e_u) (e_c may be NULL); pred_x0 = (x - sqrt(1-a_t) e)/sqrt(a_t);
  *   x_prev = sqrt(a_prev) pred_x0 + sqrt(1 - a_prev - sigma^2) e + sigma * noise (noise may be NULL). */
