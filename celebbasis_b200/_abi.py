@@ -40,6 +40,7 @@ SIGS = {
     "cb_attention_bwd_dq": [_p, _l, _p, _l, _p, _l, _p, _l, _p, _l, _p, _p, _p, _l, _p, _l, _i, _i, _i, _i, _i, _i, _f, _i, _p],
     "cb_q_sample": [_p, _p, _p, _p, _p, _p, _i, _i, _p],
     "cb_q_sample_masked": [_p, _p, _p, _p, _p, _p, _l, _l, _p, _p, _i, _i, _i, _p],
+    "cb_p_sample": [_p, _p, _p, _p, _p, _p, _p, _p, _p, _f, _i, _p, _p, _i, _i, _p],
     "cb_channel_affine_act": [_p, _i, _p, _i, _p, _p, _p, _l, _i, _p],
     "cb_face_warp_resize": [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     "cb_l2norm_rows": [_p, _p, _i, _i, _p],

@@ -281,6 +281,60 @@ __global__ void q_sample_masked_kernel(const float* __restrict__ x0, const float
     }
 }
 
+// One DDPM ancestral step for eps-prediction (LatentDiffusion.p_sample -> p_mean_variance -> predict_start_from_noise ->
+// q_posterior, ddpm.py:231-244,1118-1179), one sample of n values per blockIdx.y, t read on the device:
+//   x_recon = sr[t]*x - srm1[t]*eps  (clamped to [-1, 1] with clip);  mean = c1[t]*x_recon + c2[t]*x
+//   x_prev  = mean + ((1 - (t == 0)) * exp(0.5*lv[t])) * (noise*temperature)
+// every operation is an explicitly rounded fp32 op in the reference's evaluation order (no FMA contraction; clamp keeps
+// NaN as torch's does), so the result is bit-identical to the eager fp32 expression.  `x_prev` may alias `x` (each
+// element is read before it is written, by the same thread).
+__device__ __forceinline__ void ddpm_step(float x, float e, float nz, float sr, float srm1, float c1, float c2, float sd,
+                                          float temp, bool clip, float& xp, float& x0) {
+    float r = __fsub_rn(__fmul_rn(sr, x), __fmul_rn(srm1, e));
+    if (clip && !isnan(r)) r = fminf(fmaxf(r, -1.f), 1.f);
+    x0 = r;
+    const float mean = __fadd_rn(__fmul_rn(c1, r), __fmul_rn(c2, x));
+    xp = __fadd_rn(mean, __fmul_rn(sd, __fmul_rn(nz, temp)));
+}
+
+template <bool kVec>
+__global__ void p_sample_kernel(const float* x, const float* __restrict__ eps, const float* __restrict__ noise,
+                                const long long* __restrict__ t, const float* __restrict__ sqrt_recip_ac,
+                                const float* __restrict__ sqrt_recipm1_ac, const float* __restrict__ coef1,
+                                const float* __restrict__ coef2, const float* __restrict__ log_var, float temp,
+                                int clip, float* x_prev, float* x0_out, int n) {
+    pdl_sync();
+    const int b = blockIdx.y;
+    const long long tb = t[b];
+    const float sr = sqrt_recip_ac[tb], srm1 = sqrt_recipm1_ac[tb], c1 = coef1[tb], c2 = coef2[tb];
+    // nonzero_mask * exp(0.5 * log_variance): both (B,1,1,1) in the reference, multiplied before the noise
+    const float sd = __fmul_rn(tb == 0 ? 0.f : 1.f, expf(__fmul_rn(0.5f, log_var[tb])));
+    const bool cl = clip != 0;
+    const size_t row = (size_t)b * n;
+    if (kVec) {
+        const int n4 = n >> 2;
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += gridDim.x * blockDim.x) {
+            const float4 xv = reinterpret_cast<const float4*>(x + row)[i];
+            const float4 ev = reinterpret_cast<const float4*>(eps + row)[i];
+            const float4 nv = reinterpret_cast<const float4*>(noise + row)[i];
+            float4 o, r;
+            ddpm_step(xv.x, ev.x, nv.x, sr, srm1, c1, c2, sd, temp, cl, o.x, r.x);
+            ddpm_step(xv.y, ev.y, nv.y, sr, srm1, c1, c2, sd, temp, cl, o.y, r.y);
+            ddpm_step(xv.z, ev.z, nv.z, sr, srm1, c1, c2, sd, temp, cl, o.z, r.z);
+            ddpm_step(xv.w, ev.w, nv.w, sr, srm1, c1, c2, sd, temp, cl, o.w, r.w);
+            reinterpret_cast<float4*>(x_prev + row)[i] = o;
+            if (x0_out) reinterpret_cast<float4*>(x0_out + row)[i] = r;
+        }
+    } else {
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+            float o, r;
+            ddpm_step(x[row + i], eps[row + i], noise[row + i], sr, srm1, c1, c2, sd, temp, cl, o, r);
+            x_prev[row + i] = o;
+            if (x0_out) x0_out[row + i] = r;
+        }
+    }
+}
+
 // DDIM update with classifier-free guidance (ldm/models/diffusion/ddim.py:166-204)
 __global__ void ddim_step_kernel(const float* __restrict__ x, const float* __restrict__ e_u, const float* __restrict__ e_c,
                                  const float* __restrict__ noise, float* __restrict__ x_prev, float* __restrict__ pred_x0,
@@ -377,6 +431,31 @@ extern "C" int cb_q_sample_masked(const float* x0, const float* noise, const lon
     else
         CB_LAUNCH((q_sample_masked_kernel<false>), grid, 256, 0, st, x0, noise, t, sqrt_ac, sqrt_1mac, mask,
                   mask_bstride, mask_cstride, img, out, C, HW);
+    CB_CUDA(cudaGetLastError());
+    cb::count_launches(1);
+    return 0;
+}
+
+extern "C" int cb_p_sample(const float* x, const float* eps, const float* noise, const long long* t,
+                           const float* sqrt_recip_ac, const float* sqrt_recipm1_ac, const float* coef1,
+                           const float* coef2, const float* log_var, float temperature, int clip_denoised,
+                           float* x_prev, float* x0, int B, int n, void* stream) {
+    CB_REQUIRE(x && eps && noise && t && sqrt_recip_ac && sqrt_recipm1_ac && coef1 && coef2 && log_var && x_prev,
+               CB_ERR_ARG, "p_sample: NULL pointer");
+    CB_REQUIRE(B > 0 && B <= 65535 && n > 0, CB_ERR_ARG, "p_sample: bad shape");
+    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    const bool vec = n % 4 == 0 && al16(x) && al16(eps) && al16(noise) && al16(x_prev) && (!x0 || al16(x0));
+    const int per_block = 256 * (vec ? 4 : 1);
+    int bx = (n + per_block - 1) / per_block;
+    if (bx > 64) bx = 64;
+    dim3 grid((unsigned)bx, (unsigned)B);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (vec)
+        CB_LAUNCH((p_sample_kernel<true>), grid, 256, 0, st, x, eps, noise, t, sqrt_recip_ac, sqrt_recipm1_ac, coef1,
+                  coef2, log_var, temperature, clip_denoised, x_prev, x0, n);
+    else
+        CB_LAUNCH((p_sample_kernel<false>), grid, 256, 0, st, x, eps, noise, t, sqrt_recip_ac, sqrt_recipm1_ac, coef1,
+                  coef2, log_var, temperature, clip_denoised, x_prev, x0, n);
     CB_CUDA(cudaGetLastError());
     cb::count_launches(1);
     return 0;

@@ -3,7 +3,9 @@
 Keeps the surface main.py / main_id_embed.py / scripts/stable_txt2img.py / the DDIM sampler use (SURVEY.md §8b):
 constructor keywords of configs/stable-diffusion/aigc_id.yaml, the schedule buffers, `shared_step`, `forward`,
 `p_losses`, `apply_model`, `get_input`, `get_learned_conditioning`, `encode/decode_first_stage`, `q_sample`,
-`configure_optimizers`, `training_step`, `on_save_checkpoint`, `ema_scope`.  Every tensor operation of the step is a
+`configure_optimizers`, `training_step`, `on_save_checkpoint`, `ema_scope`, the DDPM ancestral sampler (`p_sample`,
+`p_sample_loop`, `progressive_denoising`, `sample`: one cb_p_sample launch per step) and `sample_log` / `log_images`
+with every panel an AutoencoderKL model can log.  Every tensor operation of the step is a
 kernel of libcelebbasis_b200.so reached through the mirrored sub-modules; this file is glue, exactly as in the
 reference.  Lightning is optional: without pytorch_lightning the class derives from a minimal stand-in.
 """
@@ -77,6 +79,20 @@ class _MSEFn(torch.autograd.Function):
             for b in range(ctx.B):
                 ops.axpby(grad[b].view(1, -1), w[b], out=out[b].view(1, -1))
         return out, None
+
+
+def _row_grid(images, padding=2):
+    """n decoded (b, C, H, W) batches -> one (C, b*(H+p)+p, n*(W+p)+p) image, sample k's n images along row k with
+    `padding` zero pixels around each: the reference's rearrange('n b c h w -> (b n) c h w') + torchvision make_grid
+    (nrow=n, pad_value 0) of ddpm.py:584-587,1365-1368."""
+    rows = torch.stack(images, 1)                                # b, n, C, H, W
+    b, n, C, H, W = rows.shape
+    if C == 1:
+        rows, C = rows.expand(b, n, 3, H, W), 3
+    grid = rows.new_zeros(C, b, H + padding, n, W + padding)
+    grid[:, :, padding:, :, padding:] = rows.permute(2, 0, 3, 1, 4)
+    grid = grid.reshape(C, b * (H + padding), n * (W + padding))
+    return torch.nn.functional.pad(grid, (0, padding, 0, padding))
 
 
 def _plain(cfg):
@@ -558,38 +574,208 @@ class LatentDiffusion(DDPM):
         loss_dict.update({f'{prefix}/loss': loss})
         return loss, loss_dict
 
+    # ---- DDPM ancestral sampling (ddpm.py:1118-1303) ---------------------------------------------------------------
+    def _ddpm_unsupported(self, quantize_denoised=False, return_codebook_ids=False, score_corrector=None):
+        if score_corrector is not None:
+            raise NotImplementedError("score_corrector is not supported: the reference tree ships no score corrector "
+                                      "(ddpm.py:1123-1125 calls score_corrector.modify_score)")
+        if quantize_denoised:
+            raise NotImplementedError("quantize_denoised=True is not supported: the reference calls "
+                                      "first_stage_model.quantize (ddpm.py:1139-1140), which AutoencoderKL lacks")
+        if return_codebook_ids:
+            raise NotImplementedError("return_codebook_ids=True is not supported: the reference raises "
+                                      "DeprecationWarning('Support dropped.') there (ddpm.py:1159-1160)")
+        if self.num_timesteps_cond > 1:
+            raise NotImplementedError("num_timesteps_cond > 1 (shorten_cond_schedule) is not supported: no config sets "
+                                      "it, and the reference then q-samples the conditioning every step")
+
+    @torch.no_grad()
+    def p_sample(self, x, c, t, clip_denoised=False, repeat_noise=False, return_codebook_ids=False,
+                 quantize_denoised=False, return_x0=False, temperature=1., noise_dropout=0., score_corrector=None,
+                 corrector_kwargs=None):
+        """One ancestral step x_t -> x_{t-1} (ddpm.py:1149-1178): the UNet, the noise_like draw (made at t == 0 too, as
+        the reference does), then one cb_p_sample launch for predict_start_from_noise + clamp + q_posterior + noise."""
+        self._ddpm_unsupported(quantize_denoised, return_codebook_ids, score_corrector)
+        eps = self.apply_model(x, t, c)
+        noise = noise_like(x.shape, x.device, repeat_noise)
+        if noise_dropout > 0.:
+            # the reference rounds noise * temperature before the dropout: do that here, and multiply by 1 in the kernel
+            noise = torch.nn.functional.dropout(noise * temperature, p=noise_dropout)
+            temperature = 1.
+        x_prev, x0 = ops.p_sample(x.float().contiguous(), eps.float().contiguous(), noise.float().contiguous(),
+                                  t.to(device=x.device, dtype=torch.long).contiguous(), self.sqrt_recip_alphas_cumprod,
+                                  self.sqrt_recipm1_alphas_cumprod, self.posterior_mean_coef1,
+                                  self.posterior_mean_coef2, self.posterior_log_variance_clipped,
+                                  temperature=temperature, clip_denoised=clip_denoised, want_x0=return_x0)
+        return (x_prev, x0) if return_x0 else x_prev
+
+    def _masked_blend(self, img, ts, mask, x0):
+        """img_orig = q_sample(x0, ts) (its own randn_like draw, ddpm.py:290); img_orig * mask + (1 - mask) * img in one
+        cb_q_sample_masked launch (ddpm.py:1225-1228,1274-1276).  `img` is this step's fresh output: written in place."""
+        noise = torch.randn_like(x0)
+        return ops.q_sample_masked(x0, noise, ts, self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod, mask,
+                                   img, out=img)
+
+    @staticmethod
+    def _masked_inputs(mask, x0, img):
+        if mask is None:
+            return None, x0
+        assert x0 is not None
+        assert tuple(x0.shape) == tuple(img.shape), (tuple(x0.shape), tuple(img.shape))
+        return mask.to(device=img.device, dtype=torch.float32), x0.to(img.device).float().contiguous()
+
+    @staticmethod
+    def _slice_cond(cond, batch_size):
+        """The reference's conditioning slicing to batch_size (ddpm.py:1198-1203,1293-1298)."""
+        if cond is None:
+            return None
+        if isinstance(cond, dict):
+            return {key: cond[key][:batch_size] if not isinstance(cond[key], list) else
+                    list(map(lambda x: x[:batch_size], cond[key])) for key in cond}
+        return [c[:batch_size] for c in cond] if isinstance(cond, list) else cond[:batch_size]
+
+    @torch.no_grad()
+    def progressive_denoising(self, cond, shape, verbose=True, callback=None, quantize_denoised=False,
+                              img_callback=None, mask=None, x0=None, temperature=1., noise_dropout=0.,
+                              score_corrector=None, corrector_kwargs=None, batch_size=None, x_T=None, start_T=None,
+                              log_every_t=None):
+        """ddpm.py:1180-1234: ancestral sampling that keeps the x0 predictions; `temperature` is a float or a list
+        indexed by the timestep.  Returns (x_0, [x0 prediction at every logged step])."""
+        self._ddpm_unsupported(quantize_denoised, False, score_corrector)
+        if not log_every_t:
+            log_every_t = self.log_every_t
+        timesteps = self.num_timesteps
+        if batch_size is not None:
+            b = batch_size
+            shape = [batch_size] + list(shape)
+        else:
+            b = batch_size = shape[0]
+        img = torch.randn(shape, device=self.device) if x_T is None else x_T
+        intermediates = []
+        cond = self._slice_cond(cond, batch_size)
+        if start_T is not None:
+            timesteps = min(timesteps, start_T)
+        if isinstance(temperature, (int, float)):
+            temperature = [float(temperature)] * timesteps
+        mask, x0 = self._masked_inputs(mask, x0, img)
+        for i in reversed(range(0, timesteps)):
+            ts = torch.full((b,), i, device=self.device, dtype=torch.long)
+            img, x0_partial = self.p_sample(img, cond, ts, clip_denoised=self.clip_denoised,
+                                            quantize_denoised=quantize_denoised, return_x0=True,
+                                            temperature=temperature[i], noise_dropout=noise_dropout,
+                                            score_corrector=score_corrector, corrector_kwargs=corrector_kwargs)
+            if mask is not None:
+                img = self._masked_blend(img, ts, mask, x0)
+            if i % log_every_t == 0 or i == timesteps - 1:
+                intermediates.append(x0_partial)
+            if callback:
+                callback(i)
+            if img_callback:
+                img_callback(img, i)
+        return img, intermediates
+
+    @torch.no_grad()
+    def p_sample_loop(self, cond, shape, return_intermediates=False, x_T=None, verbose=True, callback=None,
+                      timesteps=None, quantize_denoised=False, mask=None, x0=None, img_callback=None, start_T=None,
+                      log_every_t=None):
+        """ddpm.py:1236-1285: min(timesteps, start_T) ancestral steps from x_T (drawn when None), with the masked blend
+        after every step when `mask` is given.  Intermediates: x_T, then x_t at every logged step."""
+        self._ddpm_unsupported(quantize_denoised)
+        if not log_every_t:
+            log_every_t = self.log_every_t
+        device = self.betas.device
+        b = shape[0]
+        img = torch.randn(shape, device=device) if x_T is None else x_T
+        intermediates = [img]
+        if timesteps is None:
+            timesteps = self.num_timesteps
+        if start_T is not None:
+            timesteps = min(timesteps, start_T)
+        mask, x0 = self._masked_inputs(mask, x0, img)
+        for i in reversed(range(0, timesteps)):
+            ts = torch.full((b,), i, device=device, dtype=torch.long)
+            img = self.p_sample(img, cond, ts, clip_denoised=self.clip_denoised, quantize_denoised=quantize_denoised)
+            if mask is not None:
+                img = self._masked_blend(img, ts, mask, x0)
+            if i % log_every_t == 0 or i == timesteps - 1:
+                intermediates.append(img)
+            if callback:
+                callback(i)
+            if img_callback:
+                img_callback(img, i)
+        if return_intermediates:
+            return img, intermediates
+        return img
+
+    @torch.no_grad()
+    def sample(self, cond, batch_size=16, return_intermediates=False, x_T=None, verbose=True, timesteps=None,
+               quantize_denoised=False, mask=None, x0=None, shape=None, **kwargs):
+        """ddpm.py:1287-1303: p_sample_loop over (batch_size, channels, image_size, image_size) with the conditioning
+        sliced to batch_size.  Like the reference, other keywords (eta, guidance, start_T, ...) are accepted and unused."""
+        if shape is None:
+            shape = (batch_size, self.channels, self.image_size, self.image_size)
+        cond = self._slice_cond(cond, batch_size)
+        return self.p_sample_loop(cond, shape, return_intermediates=return_intermediates, x_T=x_T, verbose=verbose,
+                                  timesteps=timesteps, quantize_denoised=quantize_denoised, mask=mask, x0=x0)
+
     # ---- image logging (ddpm.py:1305-1440; called by main.ImageLogger every batch_frequency steps) --------------------
     @torch.no_grad()
     def sample_log(self, cond, batch_size, ddim, ddim_steps, **kwargs):
-        assert ddim, "the CelebBasis configs log with the DDIM sampler"
+        """DDIM samples (ddim=True) or ancestral DDPM samples over all num_timesteps (ddim=False, ddpm.py:1305-1318);
+        returns (samples, intermediates)."""
+        if not ddim:
+            return self.sample(cond=cond, batch_size=batch_size, return_intermediates=True, **kwargs)
         from ldm.models.diffusion.ddim import DDIMSampler
         shape = (self.channels, self.image_size, self.image_size)
         return DDIMSampler(self).sample(ddim_steps, batch_size, shape, cond, verbose=False, **kwargs)
+
+    def _get_denoise_row_from_list(self, samples, desc='', force_no_decoder_quantization=False):
+        """Decode every latent of `samples` and lay them out one sample per grid row (ddpm.py:578-588)."""
+        return _row_grid([self.decode_first_stage(zd.to(self.device)) for zd in samples])
 
     @torch.no_grad()
     def log_images(self, batch, N=8, n_row=4, sample=True, ddim_steps=50, ddim_eta=1., return_keys=None,
                    quantize_denoised=True, inpaint=False, plot_denoise_rows=False, plot_progressive_rows=False,
                    plot_diffusion_rows=False, **kwargs):
-        """inputs / reconstruction / rendered captions / DDIM samples (plain and with guidance 5.0) and, with inpaint, the
-        masked-sampling panels, as the reference logs them (the progressive, denoise-row and diffusion-row panels are off
-        in every CelebBasis config)."""
+        """inputs / reconstruction / rendered captions / the forward-diffusion row / samples (DDIM with ddim_steps, or
+        DDPM over all timesteps with ddim_steps=None; plain and with guidance 5.0) with their denoise row / the masked-
+        sampling panels / the progressive x0 row, as the reference logs them (ddpm.py:1320-1440)."""
         from ldm.util import log_txt_as_img
-        assert not (plot_denoise_rows or plot_progressive_rows or plot_diffusion_rows)
+        use_ddim = ddim_steps is not None
+        if sample and plot_denoise_rows and use_ddim:
+            # the reference passes the DDIM intermediates dict to _get_denoise_row_from_list, which iterates its keys
+            # and fails on the first one (str has no .to): there is no panel to reproduce
+            raise NotImplementedError("plot_denoise_rows needs ddim_steps=None (DDPM sampling): with the DDIM sampler "
+                                      "the reference's denoise row fails on the intermediates dict")
         batch = self.preprocess_batch(batch)
         log = dict()
         z, c, x, xrec, xc = self.get_input(batch, self.first_stage_key, return_first_stage_outputs=True,
                                            force_c_encode=True, return_original_cond=True, bs=N)
         c = c['caption']
         N = min(x.shape[0], N)
+        n_row = min(x.shape[0], n_row)
         log["inputs"] = x
         log["reconstruction"] = xrec
         if self.model.conditioning_key is not None and self.cond_stage_key in ["caption"]:
             log["conditioning"] = log_txt_as_img((x.shape[2], x.shape[3]), batch["caption"][:N])
+        if plot_diffusion_rows:
+            # q_sample of the first n_row latents at every logged timestep, each with its own randn_like draw
+            diffusion_row = list()
+            z_start = z[:n_row].float().contiguous()
+            for t in range(self.num_timesteps):
+                if t % self.log_every_t == 0 or t == self.num_timesteps - 1:
+                    tt = torch.full((n_row,), t, device=self.device, dtype=torch.long)
+                    noise = torch.randn_like(z_start)
+                    z_noisy = self.q_sample(x_start=z_start, t=tt, noise=noise)
+                    diffusion_row.append(self.decode_first_stage(z_noisy))
+            log["diffusion_row"] = _row_grid(diffusion_row)
         if sample:
             with self.ema_scope("Plotting"):
-                samples, _ = self.sample_log(cond=c, batch_size=N, ddim=ddim_steps is not None, ddim_steps=ddim_steps,
-                                             eta=ddim_eta)
+                samples, z_denoise_row = self.sample_log(cond=c, batch_size=N, ddim=use_ddim, ddim_steps=ddim_steps,
+                                                         eta=ddim_eta)
             log["samples"] = self.decode_first_stage(samples)
+            if plot_denoise_rows:
+                log["denoise_row"] = self._get_denoise_row_from_list(z_denoise_row)
             uc = self.get_learned_conditioning(len(c) * [""])
             sample_scaled, _ = self.sample_log(cond=c, batch_size=N, ddim=ddim_steps is not None, ddim_steps=ddim_steps,
                                                eta=ddim_eta, unconditional_guidance_scale=5.0,
@@ -611,6 +797,11 @@ class LatentDiffusion(DDPM):
                     samples, _ = self.sample_log(cond=c, batch_size=N, ddim=ddim_steps is not None, eta=ddim_eta,
                                                  ddim_steps=ddim_steps, x0=z[:N], mask=mask)
                 log["samples_outpainting"] = self.decode_first_stage(samples)
+        if plot_progressive_rows:
+            with self.ema_scope("Plotting Progressives"):
+                img, progressives = self.progressive_denoising(c, shape=(self.channels, self.image_size,
+                                                                         self.image_size), batch_size=N)
+            log["progressive_row"] = self._get_denoise_row_from_list(progressives, desc="Progressive Generation")
         if return_keys:
             if np.intersect1d(list(log.keys()), return_keys).shape[0] == 0:
                 return log

@@ -797,6 +797,22 @@ def q_sample_masked(x0, noise, t, sqrt_ac, sqrt_1mac, mask, img, out=None):
     return out
 
 
+def p_sample(x, eps, noise, t, sqrt_recip_ac, sqrt_recipm1_ac, coef1, coef2, log_var, *, temperature=1.0,
+             clip_denoised=False, out=None, want_x0=True):
+    """One DDPM ancestral step (LatentDiffusion.p_sample, eps-parameterisation, ddpm.py:1149-1178) in one launch:
+    returns (x_prev, x_recon or None).  `out` may be `x`; t is an int64 (B,) device tensor."""
+    B = x.shape[0]
+    assert x.dtype == eps.dtype == noise.dtype == torch.float32 and t.dtype == torch.long and t.shape == (B,)
+    assert x.shape == eps.shape == noise.shape and x.is_contiguous() and eps.is_contiguous() and noise.is_contiguous()
+    out = torch.empty_like(x) if out is None else out
+    assert out.shape == x.shape and out.is_contiguous()
+    x0 = torch.empty_like(x) if want_x0 else None
+    _lib.check(_L().cb_p_sample(_p(x), _p(eps), _p(noise), _p(t), _p(sqrt_recip_ac), _p(sqrt_recipm1_ac), _p(coef1),
+                                _p(coef2), _p(log_var), float(temperature), int(bool(clip_denoised)), _p(out), _p(x0),
+                                B, x.numel() // B, _st()), "cb_p_sample")
+    return out, x0
+
+
 def ddim_step(x, e_uncond, e_cond, noise, *, scale, a_t, a_prev, sigma_t, sqrt_one_minus_at, want_x0=True):
     x_prev = torch.empty_like(x)
     pred_x0 = torch.empty_like(x) if want_x0 else None

@@ -315,6 +315,18 @@ int cb_q_sample(const float* x0, const float* noise, const long long* t, const f
 int cb_q_sample_masked(const float* x0, const float* noise, const long long* t, const float* sqrt_ac,
                        const float* sqrt_1mac, const float* mask, long long mask_bstride, long long mask_cstride,
                        const float* img, float* out, int B, int C, int HW, void* stream);
+/* cb_p_sample: one DDPM ancestral step of LatentDiffusion.p_sample for eps-prediction (ddpm.py:1149-1178, through
+ *   p_mean_variance :1118-1147, predict_start_from_noise :231-235 and q_posterior :237-244); x, eps, noise, x_prev, x0
+ *   are [B][n] fp32, t is read on the device (int64, B entries), the five tables are the model's fp32 schedule buffers:
+ *     x_recon = sqrt_recip_ac[t]*x - sqrt_recipm1_ac[t]*eps, clamped to [-1, 1] when clip_denoised != 0
+ *     mean    = coef1[t]*x_recon + coef2[t]*x
+ *     x_prev  = mean + ((1 - (t == 0)) * exp(0.5*log_var[t])) * (noise*temperature)
+ *   x0 (may be NULL) receives x_recon.  x_prev may alias x.  Each operation is rounded separately, in the reference's
+ *   order: bit-identical to the eager fp32 expression.  A NULL required pointer or a non-positive size launches
+ *   nothing and returns CB_ERR_ARG. */
+int cb_p_sample(const float* x, const float* eps, const float* noise, const long long* t, const float* sqrt_recip_ac,
+                const float* sqrt_recipm1_ac, const float* coef1, const float* coef2, const float* log_var,
+                float temperature, int clip_denoised, float* x_prev, float* x0, int B, int n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * CosFace-R100 front end (no-grad): meta_net.py:253-264, iresnet.py:26-64.
