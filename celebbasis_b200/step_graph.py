@@ -26,7 +26,7 @@ from . import ops
 
 
 class StepGraphs:
-    def __init__(self, eng, B=1, T=77, n_chunks=2, image_hw=512, graphs=True):
+    def __init__(self, eng, B=1, T=77, n_chunks=2, image_hw=512):
         self.eng = eng
         dev = eng.dev
         self.B, self.T, self.n_chunks = B, T, n_chunks
@@ -49,10 +49,11 @@ class StepGraphs:
         self.ids_person = torch.zeros(B, n_chunks, dtype=torch.int64, device=dev) if faces else None
         self.loss = None
         self.outs = {}              # per graph: (loss tensor, eng.last of that capture) -- static addresses per graph
-        self.use_graphs = graphs
         self.g_pre = self.g_main = self.g_pipe = None
         self.next_token = None      # identity of the batch whose front-end result sits in (z_n, v_n)
         self.launches = {}
+        self._hi = torch.cuda.Stream(device=dev, priority=-1)     # G_pipe: the chain
+        self._lo = torch.cuda.Stream(device=dev)                  # G_pipe: the next batch's front end
 
     # ---- input staging (host or device sources; pinned host memory makes the copies asynchronous) -----------------
     def load_next(self, image, faces, posterior_eps):
@@ -82,9 +83,6 @@ class StepGraphs:
         self.loss = self.eng.stage_main(self.z, self.v, self.ids_person, self.ids, self.map, self.t, self.noise)
         self._last = dict(self.eng.last)
 
-    def _body_pre(self):
-        self._front_end()
-
     def _body_main(self):
         self._promote()
         self._chain()
@@ -92,7 +90,7 @@ class StepGraphs:
     def _body_pipe(self):
         self._promote()
         main = torch.cuda.current_stream()
-        hi, lo = self.eng._prio_stream(), self._lo_stream()
+        hi, lo = self._hi, self._lo
         fork = torch.cuda.Event()
         fork.record(main)
         hi.wait_event(fork)
@@ -108,37 +106,28 @@ class StepGraphs:
         main.wait_event(j_lo)
         main.wait_event(j_hi)
 
-    def _lo_stream(self):
-        if getattr(self, "_lo", None) is None:
-            self._lo = torch.cuda.Stream(device=self.eng.dev)
-        return self._lo
-
     # ---- capture ---------------------------------------------------------------------------------------------------
     def capture(self):
         """Eager warm-up (runs the per-shape GEMM autotuner un-captured, builds every lazily created buffer), then captures
         the three graphs.  Inputs must have been staged with load_next / load_step."""
         from . import lib
         eng = self.eng
-        eng._warm = True
         state0 = [x.clone() for x in eng.ema_state()]       # the warm-up steps move the EMA state
         for _ in range(2):
-            self._body_pre()
+            self._front_end()
             self._body_main()
         self._body_pipe()
         torch.cuda.synchronize()
         pool = None
         self.gemm_record = []       # (desc bytes, flops) of one whole step (pre + main): pointers into the graphs' pool
-        for name, body in (("pre", self._body_pre), ("main", self._body_main), ("pipe", self._body_pipe)):
+        for name, body in (("pre", self._front_end), ("main", self._body_main), ("pipe", self._body_pipe)):
             n0 = lib.launch_count()
             ops.GEMM_RECORD = [] if name != "pipe" else None
-            if self.use_graphs:
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, pool=pool):      # the graphs never run concurrently: one shared memory pool
-                    body()
-                pool = g.pool()
-                setattr(self, "g_" + name, g)
-            else:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=pool):      # the graphs never run concurrently: one shared memory pool
                 body()
+            pool = g.pool()
+            setattr(self, "g_" + name, g)
             self.launches[name] = lib.launch_count() - n0
             if ops.GEMM_RECORD is not None:
                 self.gemm_record += ops.GEMM_RECORD
@@ -150,26 +139,18 @@ class StepGraphs:
             x.copy_(x0)
         return self
 
-    def _run(self, name):
-        g = getattr(self, "g_" + name)
-        if g is not None:
-            g.replay()
-        else:
-            getattr(self, "_body_" + name)()
-
     # ---- stepping --------------------------------------------------------------------------------------------------
     def prefetch(self, token=None):
         """Front end of the batch staged in the `next` slot (prologue of the pipeline, or a step without look-ahead)."""
-        self._run("pre")
+        self.g_pre.replay()
         self.next_token = token
 
     def step(self, lookahead=False, token=None):
         """Chain on the batch whose front end was produced last (by prefetch() or by the previous step(lookahead=True));
         with lookahead=True the front end of the batch now staged in the `next` slot runs concurrently."""
         name = "pipe" if lookahead else "main"
-        self._run(name)
+        getattr(self, "g_" + name).replay()
         self.next_token = token if lookahead else None
-        if self.use_graphs:
-            self.loss, self._last = self.outs[name]
+        self.loss, self._last = self.outs[name]
         self.eng.last = self._last
         return self.loss

@@ -9,8 +9,6 @@ This is the function LatentDiffusion.shared_step + loss.backward() + optimizer.s
 (ldm/models/diffusion/ddpm.py:921-936,1069-1116,1442-1454).  Forward and backward are launched back to back so the
 whole step can be captured in one CUDA graph; torch is used for buffers, streams and the graph only.
 """
-import contextlib
-
 import numpy as np
 import torch
 
@@ -102,8 +100,7 @@ class _LatentTrainStep:
                                     res_dtype=vae_res_dtype)
         self.step_dev = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.lr = lr
-        self._side = None
-        self._warm = False
+        self._aux = torch.cuda.Stream(device=self.dev, priority=-1)     # stage_main's text branch
         self.tokenizer = tokenizer
         self.scale_factor = float(params["scale_factor"])
         # schedule (ddpm.py:126-178; util.py:21-25: float64 linspace of sqrt(beta), squared)
@@ -113,7 +110,6 @@ class _LatentTrainStep:
         self.sqrt_ac = torch.tensor(np.sqrt(ac), dtype=torch.float32, device=self.dev)
         self.sqrt_1mac = torch.tensor(np.sqrt(1.0 - ac), dtype=torch.float32, device=self.dev)
         self.num_timesteps = T
-        self._prio = None
         self.last = {}
 
     def _init_flat(self, tensors):
@@ -145,21 +141,6 @@ class _LatentTrainStep:
         """ddpm.py:289-292 per sample (the two coefficients are device scalars gathered by t)."""
         return ops.q_sample(z.contiguous(), noise.contiguous(), t.contiguous(), self.sqrt_ac, self.sqrt_1mac)
 
-    def _side_stream(self):
-        if self._side is None:
-            self._side = torch.cuda.Stream(device=self.dev)
-        return self._side
-
-    def _aux_stream(self):
-        if getattr(self, "_aux", None) is None:
-            self._aux = torch.cuda.Stream(device=self.dev, priority=-1)
-        return self._aux
-
-    def _prio_stream(self):
-        if self._prio is None:
-            self._prio = torch.cuda.Stream(device=self.dev, priority=-1)
-        return self._prio
-
     def ema_state(self):
         """Device tensors a step updates besides the gradient (restored after StepGraphs' warm-up steps)."""
         return ()
@@ -171,7 +152,7 @@ class _LatentTrainStep:
         # the text branch (rows -> inject -> 12 CLIP layers, ~110 small launches) runs beside the UNet's prefix (timestep
         # MLP, stem, first ResBlock, first self-attention): the UNet waits for the context at its first cross-attention
         main = torch.cuda.current_stream()
-        aux = self._aux_stream()
+        aux = self._aux
         fork = torch.cuda.Event()
         fork.record(main)
         aux.wait_event(fork)
@@ -219,7 +200,7 @@ class CelebBasisStep(_LatentTrainStep):
         sd = state_dict
         sub = lambda pre: {k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}
         self.face = IResNetEngine(sub("embedding_manager.meta_id_net.id_model."), self.dev, dtype=dtype)
-        self.overlap_branches = True     # VAE encode || face net + CLIP text on two streams (see run())
+        self._side = torch.cuda.Stream(device=self.dev)      # stage_prefetch's face net, beside the VAE encode
         pc = params["personalization_config"]["params"]
         self.es = pc["num_embeds_per_token"]
         self.K = pc["meta_inner_dim"]
@@ -263,73 +244,15 @@ class CelebBasisStep(_LatentTrainStep):
 
     def forward_backward(self, batch, draws, need_grad=True, ema_update=True):
         """batch: dict as face_id.py:598-644 yields (tensors on self.dev); draws: t (B,), noise, posterior_eps.
-        Returns the loss (1-element device tensor).  Gradients of (W,b) land in self.grad."""
+        Returns the loss (1-element device tensor).  Gradients of (W,b) land in self.grad.  The same two stages as the
+        serial schedule of StepGraphs, run eagerly: the front end, then the chain on its result."""
         ids, map_np, positions = self.prepare(batch["caption"])
-        ids_dev = ids.to(self.dev)
-        map_dev = torch.from_numpy(map_np).to(self.dev)
         io = batch["image_ori"]
-        return self.run(batch["image"], io["faces"], io["ids"], ids_dev, map_dev, draws["t"], draws["noise"],
-                        draws["posterior_eps"], need_grad=need_grad, ema_update=ema_update, positions=positions, ids=ids)
-
-    def run(self, image, faces, ids_person, ids_dev, map_dev, t, noise, posterior_eps, *, need_grad=True,
-            ema_update=True, positions=None, ids=None):
-        """Device side of the step: only kernel launches on the current stream (CUDA-graph capturable)."""
-        B = image.shape[0]
-        n_chunks = ids_person.shape[1]
-        T = ids_dev.shape[1]
-        # Two independent branches until the UNet: (a) face net -> celeb-basis MLP -> CLIP text (small, latency-bound
-        # launches that use few SMs) and (b) VAE encode + q_sample (large, throughput-bound convs).  They run on two
-        # streams (fork/join with events; a captured graph keeps them as parallel branches), each with its own
-        # workspace lane.
-        main = torch.cuda.current_stream()
-        overlap = self.overlap_branches and self._warm      # first call: sequential, so the GEMM autotuner times alone
-        self._warm = True
-        if overlap:
-            side = self._side_stream()
-            fork = torch.cuda.Event()
-            fork.record(main)
-            side.wait_event(fork)
-            ctx_a, lane_a = torch.cuda.stream(side), ops.lane(1)
-        else:
-            ctx_a, lane_a = contextlib.nullcontext(), contextlib.nullcontext()
-        with ctx_a, lane_a:
-            v = self.face_features(faces, n_chunks)                                  # (n_chunks*B, 512)
-            pre, coef, nrm = ops.celeb_mlp_fwd(v, self.W, self.b, self.es)
-            zc = ops.celeb_basis_fwd(coef, self.basis)                               # (F, es, 768)
-            tok = ops.embedding_gather(ids_dev.view(-1), self.clip.tok_table)
-            emb = ops.embed_inject_fwd(tok, zc.view(-1, zc.shape[-1]), map_dev.view(-1), self.clip.pos_table, B, T)
-            context = self.clip.forward(emb, B, need_grad=need_grad)                 # (B*T, 768) fp32
-            if overlap:
-                join = torch.cuda.Event()
-                join.record(side)
-        z, _ = self.encode_first_stage(image, posterior_eps)
-        noise = noise.contiguous()
-        x_noisy = self.q_sample(z, t, noise)
-        if overlap:
-            main.wait_event(join)
-        eps = self.unet.forward(x_noisy, t, context.view(B, T, -1), need_grad=need_grad)
-        loss_simple, d_eps = ops.mse_fwd_bwd(eps, noise, 1.0, want_grad=need_grad)   # (B,) per-sample losses
-        loss = loss_simple if B == 1 else loss_simple.mean(0, keepdim=True)
-        self.last = dict(z=z, context=context.view(B, T, -1), eps=eps, x_noisy=x_noisy, coef=coef, celeb_z=zc,
-                         face_feat=v, positions=positions, ids=ids)
-        if ema_update:
-            self._ema_update(zc, coef, ids_person, B)
-        if need_grad:
-            dctx = self.unet.backward(d_eps)
-            demb = self.clip.backward(dctx.view(B * T, -1))
-            dz = ops.embed_inject_bwd(demb, map_dev.view(-1), zc.shape[0] * self.es, B, T)
-            dcoef = ops.celeb_basis_bwd(dz.view(zc.shape), self.basis)
-            ops.celeb_mlp_bwd(dcoef, coef, nrm, pre, v, self.gW, self.gb)
-            self.last.update(d_eps=d_eps, dctx=dctx, demb=demb, dz=dz, dcoef=dcoef)
+        z, v = self.stage_prefetch(batch["image"], io["faces"], io["ids"].shape[1], draws["posterior_eps"])
+        loss = self.stage_main(z, v, io["ids"], ids.to(self.dev), torch.from_numpy(map_np).to(self.dev), draws["t"],
+                               draws["noise"], need_grad=need_grad, ema_update=ema_update)
+        self.last.update(positions=positions, ids=ids)
         return loss
-
-    def _ema_update(self, zc, coef, ids_person, B):
-        """_momentum_update, training branch (embedding_manager.py:484-489) for the main identity of each sample; the
-        identity index is read on the device (no host sync, CUDA-graph safe)."""
-        idx = ids_person if ids_person.is_cuda else ids_person.to(self.dev)
-        idx = idx.long()
-        ops.ema_rows(self.id_embeddings.view(self.max_ids, -1), idx, zc[:B].reshape(B, -1), self.momentum)
-        ops.ema_rows(self.id_coefficients.view(self.max_ids, -1), idx, coef[:B].reshape(B, -1), self.momentum)
 
     # ------------------------------------------------------------------------------------------
     # the step as two stages: a frozen no-grad front end that does not depend on the trained weights (and can therefore
@@ -339,7 +262,7 @@ class CelebBasisStep(_LatentTrainStep):
         """get_input's VAE encode + posterior sample (ddpm.py:702-759) and the CosFace features of the face crops
         (meta_net.py:329-346, no_grad): two concurrent branches with their own workspaces (lanes 1 / 2)."""
         main = torch.cuda.current_stream()
-        side = self._side_stream()
+        side = self._side
         fork = torch.cuda.Event()
         fork.record(main)
         side.wait_event(fork)
@@ -366,7 +289,12 @@ class CelebBasisStep(_LatentTrainStep):
         return dict(coef=saved[1], celeb_z=saved[3], face_feat=v)
 
     def _rows_ema(self, saved, ids_person, B):
-        self._ema_update(saved[3], saved[1], ids_person, B)
+        """_momentum_update, training branch (embedding_manager.py:484-489) for the main identity of each sample; the
+        identity index is read on the device (no host sync, CUDA-graph safe)."""
+        pre, coef, nrm, zc = saved
+        idx = (ids_person if ids_person.is_cuda else ids_person.to(self.dev)).long()
+        ops.ema_rows(self.id_embeddings.view(self.max_ids, -1), idx, zc[:B].reshape(B, -1), self.momentum)
+        ops.ema_rows(self.id_coefficients.view(self.max_ids, -1), idx, coef[:B].reshape(B, -1), self.momentum)
 
     def _rows_bwd(self, demb, map_dev, B, T, saved, v):
         pre, coef, nrm, zc = saved

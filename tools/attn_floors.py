@@ -1,6 +1,7 @@
 """How far is each flash-attention launch of the training step from what the H100 can do?  Records every
-ops.attention_fwd / attention_bwd_dq / attention_bwd call of one step (bs=1) -- so the shapes and paths are the ones the
-engines actually take -- groups them by (kernel, shape), replays each group alone as a CUDA graph and prints, per group:
+ops.attention_fwd / attention_bwd_dq / attention_bwd call of one step (bs=1), run as the benchmark's step runs it
+(stage_prefetch + stage_main) -- so the shapes and paths are the ones the engines actually take -- groups them by
+(kernel, shape), replays each group alone as a CUDA graph and prints, per group:
 time per call, calls per step and time per step; the algorithmic FLOP and the MMA FLOP the kernel issues (head dim
 padded to 16, PV / accumulation MMAs at N = 64 or 128, the statistics pass of the two-pass forward); the exp2 count; the
 tensor floor (989 TFLOP/s dense fp16) and the exp floor (16 exp2 per clock per SM at the card's max SM clock); the
@@ -44,7 +45,8 @@ ids_person = batch["image_ori"]["ids"].to(dev)
 
 
 def step_device():
-    return eng.run(st_["image"], st_["faces"], ids_person, ids_dev, map_dev, st_["t"], st_["noise"], st_["eps"])
+    z, v = eng.stage_prefetch(st_["image"], st_["faces"], ids_person.shape[1], st_["eps"])
+    return eng.stage_main(z, v, ids_person, ids_dev, map_dev, st_["t"], st_["noise"])
 
 
 # record the attention calls of one captured step (the graph is kept alive: its pool holds the recorded operands)

@@ -29,7 +29,7 @@ def pre(b, d):
 z1, v1 = pre(*bs[1]); z2, v2 = pre(*bs[1])
 print("G_pre twice: z", rel(z1, z2), "v", rel(v1, v2))
 # eager front end
-G.load_next(bs[1][0]["image"], bs[1][0]["image_ori"]["faces"], bs[1][1]["posterior_eps"]); G._body_pre(); torch.cuda.synchronize()
+G.load_next(bs[1][0]["image"], bs[1][0]["image_ori"]["faces"], bs[1][1]["posterior_eps"]); G._front_end(); torch.cuda.synchronize()
 print("eager vs G_pre: z", rel(G.z_n, z1), "v", rel(G.v_n, v1))
 # inside G_pipe
 pre(*bs[0])

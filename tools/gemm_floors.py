@@ -1,6 +1,7 @@
 """How far is each GEMM shape of the training step from what the H100 can do?  Records every cb_gemm descriptor of one
-step (bs=1), groups them by shape, replays each group alone as a CUDA graph and prints, per shape: time, FLOP, unique
-bytes (weights + A + D + R), the compute floor (989 TFLOP/s dense fp16) and the HBM floor (3.35 TB/s), the name of the
+step (bs=1) as the benchmark's step issues them (stage_prefetch + stage_main: the same streams and workspace lanes, so
+each descriptor carries the configuration its lane runs), groups them by shape, replays each group alone as a CUDA graph
+and prints, per shape: time, FLOP, unique bytes (weights + A + D + R), the compute floor (989 TFLOP/s dense fp16) and the HBM floor (3.35 TB/s), the name of the
 floor that bounds, the fraction of it achieved, and the launch configuration (the descriptor's autotuned tile width,
 split, ring depth and reduction path -- 0 means the library's own choice -- plus the number of CTAs the launch ran).
 
@@ -35,7 +36,8 @@ ids_person = batch["image_ori"]["ids"].to(dev)
 
 
 def step_device():
-    return eng.run(st_["image"], st_["faces"], ids_person, ids_dev, map_dev, st_["t"], st_["noise"], st_["eps"])
+    z, v = eng.stage_prefetch(st_["image"], st_["faces"], ids_person.shape[1], st_["eps"])
+    return eng.stage_main(z, v, ids_person, ids_dev, map_dev, st_["t"], st_["noise"])
 
 
 for _ in range(2):

@@ -11,7 +11,7 @@ import torch
 
 torch.backends.cuda.matmul.allow_tf32 = False
 torch.backends.cudnn.allow_tf32 = False
-from celebbasis_b200 import synth, workload
+from celebbasis_b200 import ops, synth, workload
 from celebbasis_b200.tokenizer import SyntheticCLIPTokenizer
 from celebbasis_b200.train_step import CelebBasisStep
 from oracle import torch_ref
@@ -20,6 +20,14 @@ from oracle import torch_ref
 def rel(a, b):
     a, b = a.float().cpu().flatten(), b.float().cpu().flatten()
     return ((a - b).norm() / (b.norm() + 1e-30)).item()
+
+
+def _tap(fn, out, key, pick):
+    def wrapped(*args, **kw):
+        r = fn(*args, **kw)
+        out[key] = r if pick is None else r[pick]
+        return r
+    return wrapped
 
 
 def run(kind, loss_scale=1024.0, dtype=torch.float16):
@@ -42,8 +50,18 @@ def run(kind, loss_scale=1024.0, dtype=torch.float16):
     out = om.step(bdev, ddev, ids, basis, tok.word_id("sks"))
     out["loss"].backward()
     eng = CelebBasisStep(params, sd, basis, dev, tokenizer=tok, loss_scale=loss_scale, dtype=dtype)
-    loss = eng.forward_backward(bdev, ddev)
-    L = eng.last
+    # the backward's intermediate gradients, taken from the calls that produce them: (owner, function, key, output)
+    taps = [(ops, "mse_fwd_bwd", "d_eps", 1), (eng.unet, "backward", "dctx", None), (eng.clip, "backward", "demb", None),
+            (ops, "embed_inject_bwd", "dz", None), (ops, "celeb_basis_bwd", "dcoef", None)]
+    L, originals = {}, [getattr(owner, name) for owner, name, _, _ in taps]
+    for (owner, name, key, pick), fn in zip(taps, originals):
+        setattr(owner, name, _tap(fn, L, key, pick))
+    try:
+        loss = eng.forward_backward(bdev, ddev)
+    finally:
+        for (owner, name, _, _), fn in zip(taps, originals):
+            setattr(owner, name, fn)
+    L.update(eng.last)
     rec = dict(case=f"grad_{kind}_S{loss_scale}_{str(dtype)[6:]}", loss=loss.item(), loss_ref=out["loss"].item(),
                eps_rel=rel(L["eps"], out["eps"]), ctx_rel=rel(L["context"], out["context"]),
                d_eps_rel=rel(L["d_eps"], out["eps"].grad), dctx_rel=rel(L["dctx"], out["context"].grad),

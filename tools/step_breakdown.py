@@ -1,5 +1,6 @@
-"""Device time of the step's phases, each replayed alone as a CUDA graph: VAE encode | face net + MLP + CLIP text fwd |
-UNet fwd | UNet bwd | CLIP bwd + celeb-basis bwd + AdamW."""
+"""Device time of the step's phases, each replayed alone as a CUDA graph, on the streams and workspace lanes of the
+benchmark's step: front end (stage_prefetch: VAE encode || face net) | chain (stage_main: celeb-basis MLP -> CLIP text
+|| UNet prefix -> UNet -> loss -> UNet / CLIP / celeb-basis backward -> EMA) | UNet fwd | UNet fwd + bwd | AdamW."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -21,10 +22,10 @@ image, faces = batch["image"].to(dev), batch["image_ori"]["faces"].to(dev)
 t, noise, peps = draws["t"].to(dev), draws["noise"].to(dev), draws["posterior_eps"].to(dev)
 ids, map_np, _ = eng.prepare(batch["caption"])
 ids_dev, map_dev = ids.to(dev), torch.from_numpy(map_np).to(dev)
-ids_person = batch["image_ori"]["ids"]
-B, T = 1, ids_dev.shape[1]
+ids_person = batch["image_ori"]["ids"].to(dev)
 for _ in range(2):
-    eng.run(image, faces, ids_person, ids_dev, map_dev, t, noise, peps)
+    z, v = eng.stage_prefetch(image, faces, ids_person.shape[1], peps)
+    eng.stage_main(z, v, ids_person, ids_dev, map_dev, t, noise)
     eng.optimizer_step()
 torch.cuda.synchronize()
 st = {}
@@ -44,37 +45,24 @@ def timeit(name, fn, n=3):
     print(json.dumps({"phase": name, "ms": round(ms, 3)}), flush=True)
     return g
 
-def vae():
-    st["z"], _ = eng.encode_first_stage(image, peps)
-    st["xn"] = eng.q_sample(st["z"], t, noise.contiguous())
+def front_end():
+    st["z"], st["v"] = eng.stage_prefetch(image, faces, ids_person.shape[1], peps)
 
-def face_clip():
-    v = eng.face_features(faces, ids_person.shape[1])
-    pre, coef, nrm = ops.celeb_mlp_fwd(v, eng.W, eng.b, eng.es)
-    zc = ops.celeb_basis_fwd(coef, eng.basis)
-    tok = ops.embedding_gather(ids_dev.view(-1), eng.clip.tok_table)
-    emb = ops.embed_inject_fwd(tok, zc.view(-1, zc.shape[-1]), map_dev.view(-1), eng.clip.pos_table, B, T)
-    st.update(v=v, pre=pre, coef=coef, nrm=nrm, zc=zc)
-    st["ctx"] = eng.clip.forward(emb, B, need_grad=True)
+def chain():
+    eng.stage_main(st["z"], st["v"], ids_person, ids_dev, map_dev, t, noise)
+    st["xn"], st["ctx"] = eng.last["x_noisy"], eng.last["context"]
 
 def unet_fwd():
-    st["eps"] = eng.unet.forward(st["xn"], t, st["ctx"].view(B, T, -1), need_grad=True)
+    st["eps"] = eng.unet.forward(st["xn"], t, st["ctx"], need_grad=True)
     st["loss"], st["d_eps"] = ops.mse_fwd_bwd(st["eps"], noise.contiguous(), 1.0, want_grad=True)
 
 keep = []
-keep.append(timeit("vae_encode+q_sample", vae))
-keep.append(timeit("face_net+mlp+clip_fwd", face_clip))
+keep.append(timeit("front_end", front_end))
+keep.append(timeit("chain", chain))
 # forward/backward pairs: the tape is consumed by backward, so capture fwd+bwd together and subtract
 keep.append(timeit("unet_fwd+loss", unet_fwd))
 def unet_fwd_bwd():
     unet_fwd()
-    st["dctx"] = eng.unet.backward(st["d_eps"])
+    eng.unet.backward(st["d_eps"])
 keep.append(timeit("unet_fwd+loss+unet_bwd", unet_fwd_bwd))
-def clip_fwd_bwd():
-    face_clip()
-    demb = eng.clip.backward(st["dctx"].view(B * T, -1))
-    dz = ops.embed_inject_bwd(demb, map_dev.view(-1), st["zc"].shape[0] * eng.es, B, T)
-    dcoef = ops.celeb_basis_bwd(dz.view(st["zc"].shape), eng.basis)
-    ops.celeb_mlp_bwd(dcoef, st["coef"], st["nrm"], st["pre"], st["v"], eng.gW, eng.gb)
-    eng.optimizer_step()
-keep.append(timeit("face_net+mlp+clip_fwd + clip_bwd+celeb_bwd+adamw", clip_fwd_bwd))
+keep.append(timeit("adamw", eng.optimizer_step))
