@@ -232,6 +232,8 @@ extern "C" int cb_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int
                            reinterpret_cast<uintptr_t>(dx_lp) | reinterpret_cast<uintptr_t>(gamma)) & 15u) == 0;
     if (x_dtype != CB_F32 || !aligned || M <= 0 || !ln_plan(M, C, wpr, maxq))
         return layernorm_bwd_legacy(dy, dy_dtype, x, x_dtype, gamma, mean, rstd, dx, dx_dtype, dx_lp, M, C, accumulate, stream);
+    // CB_LN_DISPATCH16 takes any other value for bf16: refuse it here, as the fallback route does
+    CB_REQUIRE(dy_dtype >= CB_F16 && dy_dtype <= CB_F32, CB_ERR_ARG, "layernorm_bwd: bad dy dtype");
     CB_REQUIRE(dx_dtype == CB_F32 || dx_dtype == dy_dtype, CB_ERR_ARG, "layernorm_bwd: dx dtype must be f32 or equal dy dtype");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     dim3 grid(ceil_div(M, 4 / wpr));

@@ -804,6 +804,9 @@ extern "C" int cb_groupnorm_fwd(const void* x, int x_dtype, void* y, int y_dtype
                                 double* ws, void* stream) {
     int rc = gn_check(N, HW, C, G);
     if (rc) return rc;
+    // checked before any launch: the streaming pair dispatches y_dtype only after its statistics kernel is launched
+    CB_REQUIRE(x_dtype >= CB_F16 && x_dtype <= CB_F32 && y_dtype >= CB_F16 && y_dtype <= CB_F32, CB_ERR_ARG,
+               "groupnorm_fwd: unsupported dtype (x %d, y %d)", x_dtype, y_dtype);
     // the streaming pair stages whole rows with cp.async.bulk, whose sizes and addresses are multiples of 16 bytes;
     // checked here, before any launch, so that a shape is accepted or refused the same way on every device
     const size_t row_bytes = (size_t)C * (x_dtype == CB_F32 ? 4 : 2);

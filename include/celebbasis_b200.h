@@ -190,6 +190,11 @@ int cb_gemm(const cb_gemm_desc* desc, void* stream);
  * (SURVEY.md §8 a29); accumulate != 0 adds into dx (residual-branch join).
  * ------------------------------------------------------------------------------------------- */
 /* cb_groupnorm_fwd: rows of x must be multiples of 16 bytes (C * sizeof(x) % 16 == 0; CB_ERR_ARG otherwise).
+ *   Statistics: fp32 partial sums of x and x^2 per group, added in fp64; variance = E[x^2] - mean^2 (one pass).  With
+ *   u = 2^-24 and a group's mean mu, variance s2: |mean_out - mu| <= K u mean|x| and |rstd_out - r| / r <=
+ *   K u (1 + mu^2 / (s2 + eps)), r = 1 / sqrt(s2 + eps): the mu^2 term is the cancellation of the one-pass variance, so
+ *   groups whose mean is large against their spread get proportionally less accurate statistics.  LayerNorm forms its
+ *   variance in two passes and has no such term.  tests/test_gpu_norm_sweep.py holds the measured K.
  * cb_groupnorm_bwd: dx_lp (optional, dtype of dy): the result is also written as a 16-bit copy -- the operand of the
  * dgrad GEMM that consumes dx next (saves a cast launch per ResBlock / transformer block of the backward pass).
  * act_silu: bit 0 = fuse SiLU; bits 8..23 = CB_GN_CTA_CAP(n); other bits are ignored. */
