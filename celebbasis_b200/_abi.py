@@ -33,6 +33,8 @@ SIGS = {
     "cb_adamw_step": [_p, _p, _p, _p, _l, _f, _f, _f, _f, _f, _i, _p, _p],
     "cb_posterior_sample": [_p, _p, _p, _i, _i, _i, _f, _p],
     "cb_loss_mean": [_p, _p, _i, _p],
+    "cb_diffusion_loss_fwd_bwd": [_p, _p, _p, _p, _p, _f, _f, _p, _p, _p, _p, _i, _i, _f, _p],
+    "cb_ti_coarse_reg": [_p, _p, _p, _p, _i, _i, _i, _f, _p],
     "cb_ddim_step": [_p, _p, _p, _p, _p, _p, _l, _f, _f, _f, _f, _f, _p],
     "cb_attention_fwd": [_p, _l, _p, _l, _p, _l, _p, _l, _p, _p, _l, _i, _i, _i, _i, _i, _i, _f, _i, _p],
     "cb_attention_bwd": [_p, _l, _p, _l, _p, _l, _p, _l, _p, _l, _p, _p, _p, _l, _p, _l, _p, _l, _i, _i, _i, _i, _i, _i, _f,
@@ -45,6 +47,7 @@ SIGS = {
     "cb_face_warp_resize": [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     "cb_l2norm_rows": [_p, _p, _i, _i, _p],
     "cb_ema_rows": [_p, _p, _i, _p, _i, _i, _i, _f, _p],
+    "cb_ema_rows_sel": [_p, _p, _p, _p, _p, _i, _i, _i, _f, _p],
     "cb_face_augment": [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     "cb_paste_resized": [_p, _i, _i, _p, _p, _i, _i, _i, _p],
     "cb_pack_conv_weight": [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],

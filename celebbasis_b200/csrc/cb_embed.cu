@@ -379,6 +379,97 @@ __global__ void loss_mean_kernel(const float* __restrict__ loss, float* __restri
     for (int b = 0; b < B; ++b) s += loss[b];
     out[0] = s / (float)B;
 }
+
+// EMA over a fixed-capacity list of n (identity slot, source row) pairs, folded in list order: entry k updates
+// table[ids[slot[k]]] with src[src_row[k]]; slot[k] < 0 is an unused entry.  One CTA per entry; as in ema_rows_kernel,
+// only the CTA of the LAST entry of an identity writes, folding every entry of that identity in order.
+__global__ void ema_rows_sel_kernel(float* __restrict__ table, const long long* __restrict__ ids,
+                                    const int* __restrict__ slot, const int* __restrict__ src_row,
+                                    const float* __restrict__ src, int n, int row, int n_rows, float m) {
+    pdl_sync();
+    const int k = blockIdx.y;
+    if (slot[k] < 0) return;
+    const long long id = ids[slot[k]];
+    if (id < 0 || id >= n_rows) return;
+    for (int k2 = k + 1; k2 < n; ++k2)
+        if (slot[k2] >= 0 && ids[slot[k2]] == id) return;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < row; i += gridDim.x * blockDim.x) {
+        float v = table[(size_t)id * row + i];
+        for (int k1 = 0; k1 <= k; ++k1)
+            if (slot[k1] >= 0 && ids[slot[k1]] == id) v = m * v + (1.f - m) * src[(size_t)src_row[k1] * row + i];
+        table[(size_t)id * row + i] = v;
+    }
+}
+
+// ---- weighted diffusion loss (ddpm.py:1084-1099), the timestep read on the device --------------------------------
+// pass 1, one CTA per sample: loss_simple[b] = mean_i (pred-target)^2 (the sum in a fixed order, as mse_fwd_bwd_kernel)
+// and d loss / d pred = 2*(pred-target)/per_sample * f_b * gscale, f_b = (lsw/exp(logvar[t_b]) + ew*lvlb[t_b]) / B
+__global__ void diffusion_loss_sample_kernel(const float* __restrict__ pred, const float* __restrict__ target,
+                                             const long long* __restrict__ t, const float* __restrict__ logvar,
+                                             const float* __restrict__ lvlb, float* __restrict__ loss_simple,
+                                             float* __restrict__ grad, int per_sample, int B, float lsw, float ew,
+                                             float gscale) {
+    pdl_sync();
+    __shared__ float red[32];
+    const int b = blockIdx.y;
+    const size_t base = (size_t)b * per_sample;
+    const long long tb = t[b];
+    const float f = (lsw / expf(logvar[tb]) + ew * lvlb[tb]) / (float)B;
+    const float gcoef = 2.f * (f / (float)per_sample) * gscale;
+    float acc = 0.f;
+    for (int i = threadIdx.x; i < per_sample; i += blockDim.x) {
+        const float d = pred[base + i] - target[base + i];
+        acc += d * d;
+        if (grad) grad[base + i] = d * gcoef;
+    }
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += red[w];
+        loss_simple[b] = s / (float)per_sample;
+    }
+}
+
+// pass 2, one thread: the batch means in sample order, in the reference's order of operations
+//   loss = lsw * mean_b(loss_simple[b]/exp(logvar[t_b]) + logvar[t_b]) + ew * loss_vlb,
+//   loss_vlb = mean_b(lvlb[t_b] * loss_simple[b])
+__global__ void diffusion_loss_batch_kernel(const float* __restrict__ loss_simple, const long long* __restrict__ t,
+                                            const float* __restrict__ logvar, const float* __restrict__ lvlb,
+                                            float* __restrict__ loss, float* __restrict__ loss_vlb, int B, float lsw,
+                                            float ew) {
+    pdl_sync();
+    float s = 0.f, v = 0.f;
+    for (int b = 0; b < B; ++b) {
+        const float lv = logvar[t[b]];
+        s += loss_simple[b] / expf(lv) + lv;
+        v += lvlb[t[b]] * loss_simple[b];
+    }
+    const float vlb = v / (float)B;
+    loss_vlb[0] = vlb;
+    loss[0] = lsw * (s / (float)B) + ew * vlb;
+}
+
+// ---- Textual Inversion coarse regulariser of one placeholder (embedding_manager.py:170-180, ddpm.py:1101-1107) -----
+// mean((P-P0)(P-P0)^T / n) over its nv rows = |S|^2 / (nv^2 n) with S = sum_i (p_i - p0_i):
+//   loss[0] += w * |S|^2 * inv;  grad_i += 2 w S inv for every row i;  inv = 1 / (nv^2 n).  One CTA of 256 threads.
+__global__ void __launch_bounds__(256)
+ti_coarse_reg_kernel(const float* __restrict__ p, const float* __restrict__ p0, float* __restrict__ grad,
+                     float* __restrict__ loss, int nv, int D, float inv, float w) {
+    pdl_sync();
+    __shared__ float red[8];
+    float acc = 0.f;
+    for (int c = threadIdx.x; c < D; c += blockDim.x) {
+        float s = 0.f;
+        for (int i = 0; i < nv; ++i) s += p[(size_t)i * D + c] - p0[(size_t)i * D + c];
+        acc += s * s;
+        const float g = 2.f * w * s * inv;
+        for (int i = 0; i < nv; ++i) grad[(size_t)i * D + c] += g;
+    }
+    const float tot = block_sum_256(acc, red);
+    if (threadIdx.x == 0) loss[0] += w * (tot * inv);
+}
 }  // namespace cb
 
 using namespace cb;
@@ -572,6 +663,47 @@ extern "C" int cb_ema_rows(float* table, const long long* idx, int idx_stride, c
 extern "C" int cb_loss_mean(const float* loss, float* out, int B, void* stream) {
     CB_REQUIRE(loss && out && B > 0, CB_ERR_ARG, "loss_mean: bad args");
     CB_LAUNCH((loss_mean_kernel), 1, 1, 0, reinterpret_cast<cudaStream_t>(stream), loss, out, B);
+    CB_CUDA(cudaGetLastError());
+    count_launches(1);
+    return 0;
+}
+
+extern "C" int cb_ema_rows_sel(float* table, const long long* ids, const int* slot, const int* src_row, const float* src,
+                               int n, int row, int n_rows, float momentum, void* stream) {
+    CB_REQUIRE(table && ids && slot && src_row && src && n > 0 && n <= 65535 && row > 0 && n_rows > 0, CB_ERR_ARG,
+               "ema_rows_sel: bad args");
+    const int gx = ceil_div(row, 256);
+    dim3 grid((unsigned)(gx < 8 ? gx : 8), (unsigned)n);
+    CB_LAUNCH((ema_rows_sel_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, ids, slot, src_row,
+              src, n, row, n_rows, momentum);
+    CB_CUDA(cudaGetLastError());
+    count_launches(1);
+    return 0;
+}
+
+extern "C" int cb_diffusion_loss_fwd_bwd(const float* pred, const float* target, const long long* t, const float* logvar,
+                                         const float* lvlb_weights, float l_simple_weight, float original_elbo_weight,
+                                         float* loss_simple, float* loss, float* loss_vlb, float* grad, int B,
+                                         int per_sample, float gscale, void* stream) {
+    CB_REQUIRE(pred && target && t && logvar && lvlb_weights && loss_simple && loss && loss_vlb, CB_ERR_ARG,
+               "diffusion_loss: NULL pointer");
+    CB_REQUIRE(B > 0 && B <= 65535 && per_sample > 0, CB_ERR_ARG, "diffusion_loss: bad shape");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    CB_LAUNCH((diffusion_loss_sample_kernel), dim3(1, B), 1024, 0, st, pred, target, t, logvar, lvlb_weights,
+              loss_simple, grad, per_sample, B, l_simple_weight, original_elbo_weight, gscale);
+    CB_LAUNCH((diffusion_loss_batch_kernel), 1, 1, 0, st, (const float*)loss_simple, t, logvar, lvlb_weights, loss,
+              loss_vlb, B, l_simple_weight, original_elbo_weight);
+    CB_CUDA(cudaGetLastError());
+    count_launches(2);
+    return 0;
+}
+
+extern "C" int cb_ti_coarse_reg(const float* rows, const float* init_rows, float* grad, float* loss, int nv, int D,
+                                int n_init, float weight, void* stream) {
+    CB_REQUIRE(rows && init_rows && grad && loss && nv > 0 && D > 0 && n_init > 0, CB_ERR_ARG, "ti_coarse_reg: bad args");
+    const float inv = 1.f / ((float)nv * (float)nv * (float)n_init);
+    CB_LAUNCH((ti_coarse_reg_kernel), 1, 256, 0, reinterpret_cast<cudaStream_t>(stream), rows, init_rows, grad, loss, nv,
+              D, inv, weight);
     CB_CUDA(cudaGetLastError());
     count_launches(1);
     return 0;

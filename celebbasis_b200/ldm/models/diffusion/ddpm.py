@@ -386,8 +386,6 @@ class LatentDiffusion(DDPM):
     def _fused_applicable(self, batch):
         if not (self.fused_step and self.training and self.cond_stage_trainable and not self.unfreeze_model):
             return False
-        if self.embedding_reg_weight > 0 or self.original_elbo_weight != 0 or self.l_simple_weight != 1.:
-            return False
         if self._textual_inversion():
             return self._ti_fused_applicable(batch)
         io = batch.get("image_ori") if isinstance(batch, dict) else None
@@ -397,8 +395,16 @@ class LatentDiffusion(DDPM):
         faces, nid = io.get("faces"), io.get("num_ids")
         if not torch.is_tensor(faces) or faces.shape[:3] != x.shape[:3] or faces.shape[-1] % 3 != 0:
             return False
-        if nid is None or not bool((torch.as_tensor(nid).cpu() == 1).all()):
-            return False           # two / three persons per prompt: the eager per-module path handles them
+        if nid is None:
+            return False
+        nid = torch.as_tensor(nid).cpu()
+        k = int(nid.max())
+        if int(nid.min()) < 1 or k > 3:
+            return False
+        if k > 1:       # k persons in a prompt: k placeholders and k identities, the second from face chunk 1 (meta[1])
+            ids = io.get("ids")
+            if ids is None or ids.shape[-1] < max(2, k) or len(self.embedding_manager.placeholder_strings) < k:
+                return False
         if getattr(self.cond_stage_model, "celeb_embeddings", None) is None:
             return False
         return next(self.model.parameters()).is_cuda
@@ -409,9 +415,9 @@ class LatentDiffusion(DDPM):
 
     def _ti_fused_applicable(self, batch):
         """Textual Inversion (v1-finetune.yaml) batches: fp32 (B, H, W, 3) images with one caption each.  Progressive
-        words change the number of injected vectors with the step counter and stay on the eager path; the manager
-        rejects per_image_tokens when it is built."""
-        if self.embedding_manager.progressive_words or not isinstance(batch, dict):
+        words only change the host-built row map from step to step; the manager rejects per_image_tokens when it is
+        built."""
+        if not isinstance(batch, dict):
             return False
         x, cap = batch.get(self.first_stage_key), batch.get(self.cond_stage_key)
         if not torch.is_tensor(x) or x.dim() != 4 or x.shape[-1] != 3 or x.dtype != torch.float32:
@@ -438,14 +444,23 @@ class LatentDiffusion(DDPM):
         B, hw = x.shape[0], x.shape[1]
         params = self._ti_params()
         dev = params[0].device
+        em = self.embedding_manager
         eng = TextualInversionStep(self._engine_params, self.state_dict(), [p.detach() for p in params], dev,
                                    tokenizer=self.cond_stage_model.tokenizer, lr=self.learning_rate)
+        self._fused_loss_weights(eng, force=self.embedding_reg_weight > 0)
+        if self.embedding_reg_weight > 0:
+            eng.set_coarse_reg(self.embedding_reg_weight,
+                               [em.initial_embeddings[k] if k in em.initial_embeddings else None
+                                for k in em.string_to_token_dict])
         # the placeholder parameters alias the engine's flat buffer: FusedAdamW, save() and the graphs see one memory
         for p, view in zip(params, eng.params):
             p.data = view
         T = getattr(self.cond_stage_model, "max_length", 77)
         G = StepGraphs(eng, B=B, T=T, n_chunks=0, image_hw=hw)
+        # the capture's row map must not advance the progressive-words counter: the step that follows does, once
+        counter = em.progressive_counter
         ids, map_np = self._ti_prepare(eng, batch[self.cond_stage_key])
+        em.progressive_counter = counter
         lat = G.noise.shape[-1]
         G.load_next(x, None, torch.zeros(B, 4, lat, lat))
         G.load_step(ids, map_np, torch.zeros(B, dtype=torch.long), torch.zeros_like(G.noise))
@@ -465,8 +480,12 @@ class LatentDiffusion(DDPM):
         lin = em.meta_id_net.stylegan_mlp.net[0]
         dev = lin.weight.device
         eng = CelebBasisStep(self._engine_params, self.state_dict(), self.cond_stage_model.celeb_embeddings, dev,
-                             tokenizer=self.cond_stage_model.tokenizer, placeholder=em.placeholder_strings[0],
+                             tokenizer=self.cond_stage_model.tokenizer, placeholder=em.placeholder_strings[:3],
                              lr=self.learning_rate, id_coefficients=em.id_coefficients, id_embeddings=em.id_embeddings)
+        self._fused_loss_weights(eng)
+        multi = self._multi_person(batch)
+        if multi:
+            eng.enable_multi_person(B, n_chunks)
         # one storage for the trainable tensors and the per-identity EMA state: the optimiser (FusedAdamW on the mirror's
         # parameters), save()/load() of the embedding manager and the graph all see the same memory
         eng.flat[: lin.weight.numel()].copy_(lin.weight.detach().reshape(-1))
@@ -477,13 +496,39 @@ class LatentDiffusion(DDPM):
         em.moved_to_device = True
         T = getattr(self.cond_stage_model, "max_length", 77)
         G = StepGraphs(eng, B=B, T=T, n_chunks=n_chunks, image_hw=hw)
-        ids, map_np, _ = eng.prepare(batch["caption"])
+        ids, map_np, _ = self._cb_prepare(eng, batch)
         lat = G.noise.shape[-1]
         G.load_next(x, faces, torch.zeros(B, 4, lat, lat))
         G.load_step(ids, map_np, torch.zeros(B, dtype=torch.long), torch.zeros_like(G.noise), batch["image_ori"]["ids"])
         G.capture()
-        self._fused, self._fused_sig = G, (B, hw, n_chunks, dev)
+        self._fused, self._fused_sig = G, (B, hw, n_chunks, dev, multi)
         return G
+
+    def _fused_loss_weights(self, eng, force=False):
+        """Non-default p_losses weights (or `force`: the coarse regulariser needs a loss buffer of its own): the step
+        computes its loss and loss_vlb with cb_diffusion_loss_fwd_bwd on the model's logvar and lvlb_weights tables (the
+        default keeps cb_mse_fwd_bwd + cb_loss_mean)."""
+        if force or self.l_simple_weight != 1. or self.original_elbo_weight != 0. or bool((self.logvar != 0).any()):
+            eng.set_loss_weights(self.l_simple_weight, self.original_elbo_weight, self.logvar, self.lvlb_weights)
+
+    def _multi_person(self, batch):
+        """True once a batch has named two or three persons: the step then keeps the multi-person map and EMA list, which
+        replay any later mix of 1/2/3-person samples.  A run that starts with single-person batches therefore captures
+        its graphs a second time at its first multi-person batch (once per run): until then the step makes exactly the
+        default configuration's launches.  The trained tensors, the EMA state and the optimiser state (kept by the
+        optimiser per parameter) carry over, since the new engine is built from the parameters the old one aliased."""
+        return bool(self._fused_sig is not None and len(self._fused_sig) == 5 and self._fused_sig[4]) or \
+            int(torch.as_tensor(batch["image_ori"]["num_ids"]).max()) > 1
+
+    def _cb_prepare(self, eng, batch):
+        """Host side of the CelebBasis step: tokenise + the bit-exact placeholder row map, and the EMA order of a
+        multi-person step."""
+        io = batch["image_ori"]
+        if eng.multi is None:
+            return eng.prepare(batch["caption"])
+        n_chunks = io["ids"].shape[1]
+        eng.load_ema_slots(eng.ema_slots(io["num_ids"], n_chunks))
+        return eng.prepare(batch["caption"], io["num_ids"], n_chunks)
 
     def _fused_shared_step(self, batch):
         ti = self._textual_inversion()
@@ -492,7 +537,8 @@ class LatentDiffusion(DDPM):
         B, hw = x.shape[0], x.shape[1]
         G = self._fused
         dev = next(self.model.parameters()).device
-        if G is None or self._fused_sig != (B, hw, 0 if ti else faces_of(batch).shape[-1] // 3, dev):
+        sig = (B, hw, 0, dev) if ti else (B, hw, faces_of(batch).shape[-1] // 3, dev, self._multi_person(batch))
+        if G is None or self._fused_sig != sig:
             G = self._fused_build(batch)
         eng = G.eng
         lat_shape = list(G.peps_n.shape)
@@ -502,15 +548,16 @@ class LatentDiffusion(DDPM):
         if ti:
             ids, map_np = self._ti_prepare(eng, batch[self.cond_stage_key])
         else:
-            ids, map_np, positions = eng.prepare(batch["caption"])    # tokenise + bit-exact placeholder row map (host)
+            ids, map_np, positions = self._cb_prepare(eng, batch)
             self.embedding_manager.last_positions = positions
         t = torch.randint(0, self.num_timesteps, (B,), device=dev).long()
         noise = torch.randn_like(G.z)
         G.load_step(ids, map_np, t, noise, None if ti else batch["image_ori"]["ids"])
         nxt, self._staged_next = self._staged_next, None
         if nxt is not None and (nxt is batch or not self._fused_applicable(nxt)
-                                or nxt[self.first_stage_key].shape != x.shape):
-            nxt = None
+                                or nxt[self.first_stage_key].shape != x.shape
+                                or (not ti and self._multi_person(nxt) != sig[4])):
+            nxt = None      # (a batch that switches the step to multi-person prompts has its front end run by the new graphs)
         if nxt is not None:
             G.load_next(nxt[self.first_stage_key], faces_of(nxt), torch.randn(lat_shape))
         loss_dev = G.step(lookahead=nxt is not None, token=nxt)
@@ -520,9 +567,11 @@ class LatentDiffusion(DDPM):
             lin = self.embedding_manager.meta_id_net.stylegan_mlp.net[0]
             loss = _FusedLossFn.apply(loss_dev, (eng.gW, eng.gb), lin.weight, lin.bias)
         loss_simple = eng.last["loss_simple"].detach()
+        loss_vlb = eng.last["loss_vlb"]
         prefix = 'train' if self.training else 'val'
         loss_dict = {f'{prefix}/loss_simple': loss_simple.mean(),
-                     f'{prefix}/loss_vlb': (self.lvlb_weights.to(dev)[t] * loss_simple).mean(),
+                     f'{prefix}/loss_vlb': (self.lvlb_weights.to(dev)[t] * loss_simple).mean() if loss_vlb is None
+                     else loss_vlb.detach()[0],
                      f'{prefix}/loss_emb_reg': self.embedding_manager.embedding_neg_loss(),
                      f'{prefix}/loss': loss.detach()}
         return loss, loss_dict
@@ -560,12 +609,13 @@ class LatentDiffusion(DDPM):
         logvar_t = self.logvar[t]
         loss = loss_simple / torch.exp(logvar_t) + logvar_t
         loss = self.l_simple_weight * loss.mean()
-        loss_vlb = (self.lvlb_weights[t] * loss_simple.detach()).mean()
+        loss_vlb = (self.lvlb_weights[t] * loss_simple).mean()
         loss_dict.update({f'{prefix}/loss_vlb': loss_vlb})
         loss = loss + self.original_elbo_weight * loss_vlb
         loss_dict.update({f'{prefix}/loss': loss})
         if self.embedding_reg_weight > 0:
             reg = self.embedding_manager.embedding_to_coarse_loss()
+            reg = reg.mean() if torch.is_tensor(reg) else reg       # (nv, nv) for Textual Inversion: the reference's mean
             loss_dict.update({f'{prefix}/loss_emb_reg': reg})
             loss = loss + self.embedding_reg_weight * reg
         neg = self.embedding_manager.embedding_neg_loss()

@@ -686,6 +686,18 @@ def ema_rows(table, idx, src, momentum):
                "cb_ema_rows")
 
 
+def ema_rows_sel(table, ids, slot, src_row, src, momentum):
+    """For k in list order: table[ids.view(-1)[slot[k]]] = m*table[..] + (1-m)*src[src_row[k]]; slot[k] < 0 skips entry k
+    (cb_ema_rows_sel).  ids: contiguous device int64; slot / src_row: device int32 (n,)."""
+    n = slot.numel()
+    row = src[0].numel()
+    assert ids.dtype == torch.int64 and ids.is_contiguous() and slot.dtype == torch.int32 and src_row.dtype == torch.int32
+    assert src_row.numel() == n and table.dtype == torch.float32 and src.dtype == torch.float32
+    assert table.is_contiguous() and src.is_contiguous() and table[0].numel() == row
+    _lib.check(_L().cb_ema_rows_sel(_p(table), _p(ids), _p(slot), _p(src_row), _p(src), n, row, table.shape[0],
+                                    float(momentum), _st()), "cb_ema_rows_sel")
+
+
 def embedding_gather(ids, table):
     n = ids.numel()
     out = torch.empty(n, table.shape[1], dtype=torch.float32, device=table.device)
@@ -756,6 +768,37 @@ def loss_mean(loss):
     out = torch.empty(1, dtype=torch.float32, device=loss.device)
     _lib.check(_L().cb_loss_mean(_p(loss), _p(out), loss.shape[0], _st()), "cb_loss_mean")
     return out
+
+
+def diffusion_loss_fwd_bwd(pred, target, t, logvar, lvlb_weights, l_simple_weight, original_elbo_weight, gscale=1.0,
+                           want_grad=True):
+    """p_losses with its loss weights (cb_diffusion_loss_fwd_bwd).  t: device int64 (B,); logvar / lvlb_weights: device
+    fp32 (T,).  Returns (loss_simple [B], loss [1], loss_vlb [1], d loss / d pred * gscale or None)."""
+    assert pred.dtype == torch.float32 and target.dtype == torch.float32 and t.dtype == torch.int64
+    assert pred.shape == target.shape and pred.is_contiguous() and target.is_contiguous()
+    B = pred.shape[0]
+    assert t.shape == (B,) and t.is_contiguous()
+    assert logvar.dtype == torch.float32 and lvlb_weights.dtype == torch.float32
+    assert logvar.dim() == 1 and logvar.shape == lvlb_weights.shape and logvar.is_contiguous() and lvlb_weights.is_contiguous()
+    # t is read on the device (a host check would sync): the tables must cover every timestep the schedule draws
+    loss_simple = torch.empty(B, dtype=torch.float32, device=pred.device)
+    out = torch.empty(2, dtype=torch.float32, device=pred.device)
+    grad = torch.empty_like(pred) if want_grad else None
+    _lib.check(_L().cb_diffusion_loss_fwd_bwd(_p(pred), _p(target), _p(t), _p(logvar), _p(lvlb_weights),
+                                              float(l_simple_weight), float(original_elbo_weight), _p(loss_simple),
+                                              _p(out[0:1]), _p(out[1:2]), _p(grad), B, pred.numel() // B, gscale, _st()),
+               "cb_diffusion_loss_fwd_bwd")
+    return loss_simple, out[0:1], out[1:2], grad
+
+
+def ti_coarse_reg(rows, init_rows, grad, loss, n_init, weight):
+    """loss += weight * mean((rows-init)(rows-init)^T / n_init); grad += its gradient (cb_ti_coarse_reg).  rows, init_rows
+    and grad are (nv, D) fp32 views; loss a (1,) fp32 tensor."""
+    assert rows.shape == init_rows.shape == grad.shape and rows.is_contiguous() and init_rows.is_contiguous()
+    assert grad.is_contiguous() and loss.dtype == torch.float32
+    nv, D = rows.shape
+    _lib.check(_L().cb_ti_coarse_reg(_p(rows), _p(init_rows), _p(grad), _p(loss), nv, D, int(n_init), float(weight),
+                                     _st()), "cb_ti_coarse_reg")
 
 
 def posterior_sample(moments_nchw, eps, scale):

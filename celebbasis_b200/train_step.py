@@ -111,6 +111,14 @@ class _LatentTrainStep:
         self.sqrt_1mac = torch.tensor(np.sqrt(1.0 - ac), dtype=torch.float32, device=self.dev)
         self.num_timesteps = T
         self.last = {}
+        self.loss_weights = None        # (l_simple_weight, original_elbo_weight, logvar (T,), lvlb_weights (T,))
+
+    def set_loss_weights(self, l_simple_weight, original_elbo_weight, logvar, lvlb_weights):
+        """p_losses' loss weights (ddpm.py:1084-1099).  logvar / lvlb_weights: the model's (T,) tables.  Once set, the step
+        computes its loss and gradient with cb_diffusion_loss_fwd_bwd instead of cb_mse_fwd_bwd + cb_loss_mean."""
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        self.loss_weights = (float(l_simple_weight), float(original_elbo_weight),
+                             logvar.detach().to(**f32).contiguous(), lvlb_weights.detach().to(**f32).contiguous())
 
     def _init_flat(self, tensors):
         """The trainable tensors live in ONE flat fp32 buffer (what the data-parallel all-reduce and AdamW operate on);
@@ -167,17 +175,28 @@ class _LatentTrainStep:
         x_noisy = self.q_sample(z, t, noise)
         eps = self.unet.forward(x_noisy, t, context.view(B, T, -1), need_grad=need_grad, context_ready=ctx_ready)
         main.wait_event(ctx_ready)      # (already implied by the UNet's first cross-attention; explicit for the EMA / backward)
-        loss_simple, d_eps = ops.mse_fwd_bwd(eps, noise, 1.0, want_grad=need_grad)
-        loss = loss_simple if B == 1 else ops.loss_mean(loss_simple)
+        loss_vlb = None
+        if self.loss_weights is None:
+            loss_simple, d_eps = ops.mse_fwd_bwd(eps, noise, 1.0, want_grad=need_grad)
+            loss = loss_simple if B == 1 else ops.loss_mean(loss_simple)
+        else:
+            lsw, ew, logvar, lvlb = self.loss_weights
+            loss_simple, loss, loss_vlb, d_eps = ops.diffusion_loss_fwd_bwd(eps, noise, t, logvar, lvlb, lsw, ew, 1.0,
+                                                                            want_grad=need_grad)
         self.last = dict(z=z, context=context.view(B, T, -1), eps=eps, x_noisy=x_noisy, loss_simple=loss_simple,
-                         **self._rows_last(saved, v))
+                         loss_vlb=loss_vlb, **self._rows_last(saved, v))
         if ema_update:
             self._rows_ema(saved, ids_person, B)
         if need_grad:
             dctx = self.unet.backward(d_eps)
             demb = self.clip.backward(dctx.view(B * T, -1))
             self._rows_bwd(demb, map_dev, B, T, saved, v)
+            self._loss_extra(loss)
         return loss
+
+    def _loss_extra(self, loss):
+        """Terms of the loss on the trained tensors alone, added to `loss` and to the gradient after the backward."""
+        pass
 
     def _rows_last(self, saved, v):
         return {}
@@ -210,7 +229,12 @@ class CelebBasisStep(_LatentTrainStep):
             [sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.weight"],
              sd["embedding_manager.meta_id_net.stylegan_mlp.net.0.bias"]])
         self.basis = basis.detach().to(self.dev, torch.float32).contiguous()
-        self.placeholder_token = int(tokenizer(placeholder)["input_ids"][0, 1])
+        # placeholder: the main identity's string, or the strings of the first, second and third person of a prompt
+        # (EmbeddingManagerId.placeholder_strings[:3])
+        strings = [placeholder] if isinstance(placeholder, str) else list(placeholder)[:3]
+        self.placeholder_tokens = [int(tokenizer(s)["input_ids"][0, 1]) for s in strings]
+        self.placeholder_token = self.placeholder_tokens[0]
+        self.multi = None           # multi-person EMA lists (enable_multi_person)
         # per-identity EMA side state, initialised as EmbeddingManagerId does (embedding_manager.py:229-252): ONE randn
         # coefficient tensor shared by every identity, embeddings = the initializer word's token embedding
         self.test_mode = pc.get("test_mode", "coefficient")
@@ -236,18 +260,65 @@ class CelebBasisStep(_LatentTrainStep):
         return ops.l2norm_rows(feat)
 
     # ------------------------------------------------------------------------------------------
-    def prepare(self, captions):
-        """Host side of the step: tokenise, locate the placeholder, build the row map (bit-exact integer path)."""
+    @staticmethod
+    def person_chunks(n_chunks):
+        """Face chunk of the first, second and third person of a prompt (embedding_manager.py:298-304): the injected
+        rows come from meta[0], meta[1], meta[id_cnt // 2], the EMA coefficients from cef[0], cef[1], cef[1]
+        ("in training, the max #id is 2")."""
+        return (0, 1, n_chunks // 2), (0, 1, 1)
+
+    def prepare(self, captions, num_ids=None, n_chunks=None):
+        """Host side of the step: tokenise, locate the placeholders, build the row map (bit-exact integer path).  Without
+        num_ids every prompt has one person (the main identity, face chunk 0); with the per-sample num_ids (1, 2 or 3)
+        sample b's j-th placeholder takes the rows of face chunk person_chunks(n_chunks)[0][j]."""
         ids = self.tokenize(captions)
-        map_np, positions = build_inject_map(ids.numpy(), self.placeholder_token, self.es, lambda b: b)
+        if num_ids is None:
+            map_np, positions = build_inject_map(ids.numpy(), self.placeholder_token, self.es, lambda b: b)
+            return ids, map_np, positions
+        B = ids.shape[0]
+        chunk = self.person_chunks(n_chunks)[0]
+        nid = [int(k) for k in num_ids]
+        assert all(1 <= k <= len(self.placeholder_tokens) for k in nid), (nid, len(self.placeholder_tokens))
+        per_sample = [(self.placeholder_tokens[:k], [(chunk[j] * B + b) * self.es for j in range(k)])
+                      for b, k in enumerate(nid)]
+        map_np, positions = build_inject_map_multi(ids.numpy(), per_sample, self.es)
         return ids, map_np, positions
+
+    @staticmethod
+    def ema_slots(num_ids, n_chunks):
+        """The EMA update order of a multi-person batch (embedding_manager.py:321-392: per sample, then its first, second,
+        third person) as a fixed-capacity (3B,) list: entry 3b+j is the index of ids[b][j] in the flat (B, n_chunks)
+        identity tensor, -1 where sample b has fewer than j+1 persons."""
+        nid = [int(k) for k in num_ids]
+        slot = np.full(3 * len(nid), -1, dtype=np.int32)
+        for b, k in enumerate(nid):
+            slot[3 * b: 3 * b + k] = b * n_chunks + np.arange(k)
+        return slot
+
+    def enable_multi_person(self, B, n_chunks):
+        """Steps from now on take batches whose prompts name one, two or three persons (num_ids per sample): the
+        row map comes from prepare(captions, num_ids, n_chunks) and the EMA runs over the list load_ema_slots stages,
+        so a captured step replays any mix of 1/2/3-person samples."""
+        assert n_chunks >= 2, "two- and three-person prompts take their second identity from face chunk 1"
+        emb_chunk, coef_chunk = self.person_chunks(n_chunks)
+        src = lambda chunk: torch.tensor([chunk[j] * B + b for b in range(B) for j in range(3)], dtype=torch.int32,
+                                         device=self.dev)
+        self.multi = dict(B=B, n_chunks=n_chunks, slot=torch.full((3 * B,), -1, dtype=torch.int32, device=self.dev),
+                          src_emb=src(emb_chunk), src_coef=src(coef_chunk))
+
+    def load_ema_slots(self, slot):
+        self.multi["slot"].copy_(torch.from_numpy(slot), non_blocking=True)
 
     def forward_backward(self, batch, draws, need_grad=True, ema_update=True):
         """batch: dict as face_id.py:598-644 yields (tensors on self.dev); draws: t (B,), noise, posterior_eps.
         Returns the loss (1-element device tensor).  Gradients of (W,b) land in self.grad.  The same two stages as the
         serial schedule of StepGraphs, run eagerly: the front end, then the chain on its result."""
-        ids, map_np, positions = self.prepare(batch["caption"])
         io = batch["image_ori"]
+        if self.multi is None:
+            ids, map_np, positions = self.prepare(batch["caption"])
+        else:
+            ids, map_np, positions = self.prepare(batch["caption"], io["num_ids"], io["ids"].shape[1])
+            self.load_ema_slots(self.ema_slots(io["num_ids"], io["ids"].shape[1]))
         z, v = self.stage_prefetch(batch["image"], io["faces"], io["ids"].shape[1], draws["posterior_eps"])
         loss = self.stage_main(z, v, io["ids"], ids.to(self.dev), torch.from_numpy(map_np).to(self.dev), draws["t"],
                                draws["noise"], need_grad=need_grad, ema_update=ema_update)
@@ -293,6 +364,14 @@ class CelebBasisStep(_LatentTrainStep):
         identity index is read on the device (no host sync, CUDA-graph safe)."""
         pre, coef, nrm, zc = saved
         idx = (ids_person if ids_person.is_cuda else ids_person.to(self.dev)).long()
+        if self.multi is not None:
+            mp, F = self.multi, zc.shape[0]
+            idx = idx.contiguous()
+            ops.ema_rows_sel(self.id_embeddings.view(self.max_ids, -1), idx, mp["slot"], mp["src_emb"],
+                             zc.reshape(F, -1), self.momentum)
+            ops.ema_rows_sel(self.id_coefficients.view(self.max_ids, -1), idx, mp["slot"], mp["src_coef"],
+                             coef.reshape(F, -1), self.momentum)
+            return
         ops.ema_rows(self.id_embeddings.view(self.max_ids, -1), idx, zc[:B].reshape(B, -1), self.momentum)
         ops.ema_rows(self.id_coefficients.view(self.max_ids, -1), idx, coef[:B].reshape(B, -1), self.momentum)
 
@@ -353,6 +432,23 @@ class TextualInversionStep(_LatentTrainStep):
         self.params, self.grads = self._init_flat(list(placeholder_params))
         self.rows = self.flat.view(-1, self.clip.hidden)
         self.grad_rows = self.grad.view(-1, self.clip.hidden)
+        self.coarse_reg = None
+
+    def set_coarse_reg(self, weight, initial_rows):
+        """embedding_reg_weight > 0 (ddpm.py:1101-1107): initial_rows[k] is the initial (nv, 768) rows of the k-th
+        placeholder (the engine's parameter order), or None for a placeholder without an initializer word.  The loss
+        weights must have been set (set_loss_weights, default values included): the regulariser adds into the loss buffer
+        of cb_diffusion_loss_fwd_bwd, not into loss_simple."""
+        assert self.loss_weights is not None, "set_loss_weights before set_coarse_reg"
+        terms = [(p, g, p0.detach().to(self.dev, torch.float32).reshape(p.shape).contiguous())
+                 for p, g, p0 in zip(self.params, self.grads, initial_rows) if p0 is not None]
+        self.coarse_reg = (float(weight), len(terms), terms) if terms else None
+
+    def _loss_extra(self, loss):
+        if self.coarse_reg is not None:
+            w, n_init, terms = self.coarse_reg
+            for p, g, p0 in terms:
+                ops.ti_coarse_reg(p, p0, g, loss, n_init, w)
 
     def stage_prefetch(self, image, faces, n_chunks, posterior_eps, z_out=None, v_out=None):
         """get_input's VAE encode + posterior sample (ddpm.py:702-759); there are no face crops."""

@@ -124,3 +124,35 @@ def synth_face_files(out_dir, n=4, hw=64, seed=0):
     with open(pk, "wb") as f:
         pickle.dump(paths, f)
     return pk, paths
+
+
+PERSON_CAPTIONS = {1: "a photo of a face of sks person", 2: "a photo of sks person and ks person",
+                   3: "a photo of sks and ks and ata together"}
+PERSON_MIX = ([1, 2], [3, 1], [2, 3], [1, 1], [3, 2], [2, 2], [1, 3], [2, 1])
+TI_OPTION_CAPTIONS = ["a photo of *", "a photo of sks and *", "a sks photo", "* in a photo of sks"]
+
+
+def synth_persons_batch(step, B=2, id_cnt=4, seed=11, hw=64):
+    """A CelebBasis batch whose prompts name 1, 2 or 3 persons (PERSON_MIX[step]): `id_cnt` face crops and identities
+    per sample, identity 3 shared by both samples as their second person, so the EMA order matters."""
+    g = torch.Generator().manual_seed(seed + 7919 * step)
+    image = torch.rand(B, hw, hw, 3, generator=g) * 2 - 1
+    faces = torch.rand(B, hw, hw, 3 * id_cnt, generator=g) * 2 - 1
+    ids = torch.stack([torch.randperm(10, generator=g)[:id_cnt] for _ in range(B)])
+    ids[:, 1] = 3
+    nid = torch.tensor(PERSON_MIX[step % len(PERSON_MIX)][:B], dtype=torch.long)
+    return {"image": image, "caption": [PERSON_CAPTIONS[int(k)] for k in nid],
+            "image_ori": {"faces": faces, "ids": ids, "num_ids": nid}}
+
+
+def synth_ti_option_batch(step, B=2, seed=5, hw=64):
+    """A Textual Inversion batch naming the placeholders '*' and 'sks' (two per prompt at most)."""
+    g = torch.Generator().manual_seed(seed + 7919 * step)
+    return {"image": torch.rand(B, hw, hw, 3, generator=g) * 2 - 1,
+            "caption": [TI_OPTION_CAPTIONS[(step + b) % len(TI_OPTION_CAPTIONS)] for b in range(B)]}
+
+
+def option_draws(step, B=2, lat=8, seed=41):
+    g = torch.Generator().manual_seed(seed + step)
+    return {"t": torch.tensor([0, 999]) if step == 0 else torch.randint(0, 1000, (B,), generator=g).long(),
+            "noise": torch.randn(B, 4, lat, lat, generator=g), "posterior_eps": torch.randn(B, 4, lat, lat, generator=g)}

@@ -302,6 +302,27 @@ int cb_posterior_sample(const float* moments, const float* eps, float* z, int N,
 /* cb_loss_mean: out[0] = (loss[0] + ... + loss[B-1]) / B, added in sample order: the batch mean of the per-sample
  *   losses (ddpm.py:1084-1096) inside a captured training step. */
 int cb_loss_mean(const float* loss, float* out, int B, void* stream);
+/* cb_diffusion_loss_fwd_bwd: LatentDiffusion.p_losses with its loss weights (ddpm.py:1084-1099), replacing
+ *   loss_simple = get_loss(...).mean([1,2,3]); loss = loss_simple/exp(logvar[t]) + logvar[t];
+ *   loss = l_simple_weight * loss.mean(); loss_vlb = (lvlb_weights[t] * loss_simple).mean();
+ *   loss += original_elbo_weight * loss_vlb
+ * with t read on the device (int64, B entries; logvar and lvlb_weights are fp32 tables indexed by it), so a captured
+ * step replays with a new t.  pred / target / grad are [B][per_sample] fp32; loss_simple is [B], loss and loss_vlb one
+ * float each.  grad (may be NULL) = d loss / d pred * gscale: sample b's factor
+ * (l_simple_weight/exp(logvar[t_b]) + original_elbo_weight*lvlb_weights[t_b]) / B is folded into 2*(pred-target)/per_sample.
+ * Every sum is taken in a fixed order (the batch means in sample order): bit-reproducible.  Two launches. */
+int cb_diffusion_loss_fwd_bwd(const float* pred, const float* target, const long long* t, const float* logvar,
+                              const float* lvlb_weights, float l_simple_weight, float original_elbo_weight,
+                              float* loss_simple, float* loss, float* loss_vlb, float* grad, int B, int per_sample,
+                              float gscale, void* stream);
+/* cb_ti_coarse_reg: the Textual Inversion coarse regulariser of ONE placeholder, weighted (embedding_manager.py:170-180
+ *   embedding_to_coarse_loss, ddpm.py:1101-1107 `loss += embedding_reg_weight * loss_embedding_reg.mean()`).  rows and
+ *   init_rows are the placeholder's nv trained and initial rows of D floats; n_init = len(initial_embeddings).  With
+ *   S = sum_i (rows_i - init_rows_i), mean((P-P0)(P-P0)^T / n_init) = |S|^2 / (nv^2 n_init), so
+ *     loss[0] += weight * |S|^2 / (nv^2 n_init);   grad_i += 2 weight S / (nv^2 n_init) for each of the nv rows.
+ *   One launch per placeholder with an initializer word, after the step's other gradient writes. */
+int cb_ti_coarse_reg(const float* rows, const float* init_rows, float* grad, float* loss, int nv, int D, int n_init,
+                     float weight, void* stream);
 /* cb_ddim_step: one DDIM update with classifier-free guidance, ldm/models/diffusion/ddim.py:166-204:
  *   e = e_u + s*(e_c - e_u) (e_c may be NULL); pred_x0 = (x - sqrt(1-a_t) e)/sqrt(a_t);
  *   x_prev = sqrt(a_prev) pred_x0 + sqrt(1 - a_prev - sigma^2) e + sigma * noise (noise may be NULL). */
@@ -354,6 +375,13 @@ int cb_l2norm_rows(const float* x, float* y, int rows, int D, void* stream);
  * indices outside [0, n_rows) are skipped (the reference's `if id_idx < len(self.id_embeddings)`). */
 int cb_ema_rows(float* table, const long long* idx, int idx_stride, const float* src, int B, int row, int n_rows,
                 float momentum, void* stream);
+/* cb_ema_rows_sel: the same update over a fixed-capacity list of n entries, for two- and three-person prompts
+ * (embedding_manager.py:321-392: per sample, then its first, second and third identity).  Entry k folds
+ * src[src_row[k]] into table[ids[slot[k]]]; slot[k] < 0 marks an unused entry, identities outside [0, n_rows) are
+ * skipped, and entries of one identity fold in list order.  ids is the device (B, n_chunks) int64 identity tensor, so
+ * a captured step replays with new identities and a new slot list. */
+int cb_ema_rows_sel(float* table, const long long* ids, const int* slot, const int* src_row, const float* src, int n,
+                    int row, int n_rows, float momentum, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * cb_attention_fwd -- fused softmax(Q K^T * scale [+ causal mask]) V with wgmma (flash style): the scores live in
