@@ -52,6 +52,12 @@ SIGS = {
     "cb_paste_resized": [_p, _i, _i, _p, _p, _i, _i, _i, _p],
     "cb_pack_conv_weight": [_p, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     "cb_convert_f32": [_p, _p, _i, _l, _f, _p],
+    "cb_conv_wgrad_ws_bytes": [_i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
+    "cb_conv_wgrad": [_p, _l, _p, _l, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _p, _p, _p, _l, _p],
+    "cb_colsum": [_p, _i, _l, _p, _l, _i, _i, _f, _p],
+    "cb_groupnorm_affine_bwd": [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _f, _p],
+    "cb_layernorm_affine_bwd": [_p, _i, _p, _i, _p, _p, _p, _p, _i, _i, _f, _p],
+    "cb_embedding_bwd": [_p, _p, _l, _p, _i, _i, _i, _f, _p],
 }
 
 

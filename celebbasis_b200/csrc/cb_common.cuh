@@ -41,6 +41,13 @@ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 int device_sm_count();
+// cb_gemm split-K workspace (cb_gemm.cu): bytes a launch of `splits` k-slices over m_tiles 128-row tiles of N columns and
+// `batch` batches needs (counters, then one fp32 partial-tile slice per k-slice); 0 for splits <= 1, -1 when the tile count
+// exceeds the counters (cb_gemm then never splits).  Callers that size a workspace for cb_gemm use this, not a copy of it.
+constexpr long long kSplitkCounterBytes = 65536;
+long long gemm_splitk_ws_bytes(int N, int m_tiles, int batch, int splits);
+// the slice count cb_gemm runs when `requested` (1..kiters) slices of a k-loop of `kiters` iterations are asked for
+int gemm_split_count(int kiters, int requested);
 // one-warp-per-row LayerNorm (cb_norm.cu): fallback of the vectorised kernels in cb_layernorm.cu
 int layernorm_fwd_legacy(const void* x, int x_dtype, void* y, int y_dtype, const float* gamma, const float* beta, int M,
                          int C, float eps, float* mean_out, float* rstd_out, void* stream);
@@ -271,6 +278,11 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 __device__ __forceinline__ float quick_gelu_f(float x) { return x / (1.0f + __expf(-1.702f * x)); }
 __device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+// d silu(z) / dz
+__device__ __forceinline__ float silu_grad(float z) {
+    const float s = __fdividef(1.0f, 1.0f + __expf(-z));
+    return s * (1.0f + z * (1.0f - s));
+}
 
 template <typename T> struct cvt;
 template <> struct cvt<__half> {

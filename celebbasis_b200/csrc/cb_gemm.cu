@@ -854,6 +854,15 @@ static int pick_bn(const cb_gemm_desc& d, int m_tiles, int kiters, bool requeste
     return best;
 }
 
+long long gemm_splitk_ws_bytes(int N, int m_tiles, int batch, int splits) {
+    // bounds valid for every tile width: tiles <= ceil(N / 64) * ..., tiles * BN <= (N + 255) * ...
+    if ((long long)ceil_div(N, 64) * m_tiles * batch > kSplitkCounterBytes / 4) return -1;
+    if (splits <= 1) return 0;
+    return kSplitkCounterBytes + (long long)(N + 255) * m_tiles * batch * BM * 4 * splits;
+}
+
+int gemm_split_count(int kiters, int requested) { return ceil_div(kiters, ceil_div(kiters, requested)); }
+
 }  // namespace cb
 
 using namespace cb;
@@ -1045,12 +1054,7 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
         // bit-identical whichever configuration wins the timing.
         const int bn_s = pick_bn(d, m_tiles, kiters, false);
         const long long tiles_s = (long long)ceil_div(d.N, bn_s) * m_tiles * d.batch;
-        const long long counters_bytes = 65536;
-        const long long avail = d.splitk_ws_bytes - counters_bytes;
-        // workspace bounds valid for every tile width: tiles <= ceil(N / 64) * ..., tiles * BN <= (N + 255) * ...
-        const long long tiles_max = (long long)ceil_div(d.N, 64) * m_tiles * d.batch;
-        const long long slice_bytes = (long long)(d.N + 255) * m_tiles * d.batch * BM * 4;
-        if (d.splitk_ws != nullptr && !d.glu && tiles_max <= counters_bytes / 4 &&
+        if (d.splitk_ws != nullptr && !d.glu && gemm_splitk_ws_bytes(d.N, m_tiles, d.batch, 2) > 0 &&
             (d.splits > 0 || (tiles_s < sms && kiters >= 8))) {
             const double out_elems = (double)p.M * d.batch * d.N;
             double best_t = tile_time_us(bn_s, tiles_s, kiters, sms);
@@ -1068,12 +1072,12 @@ extern "C" int cb_gemm(const cb_gemm_desc* dp, void* stream) {
             }
             if (best_sp > 1) {
                 const int per = ceil_div(kiters, best_sp);
-                const int splits = ceil_div(kiters, per);
-                if (slice_bytes * splits <= avail) {                       // one partial-tile slice per k-slice
+                const int splits = gemm_split_count(kiters, best_sp);       // ceil_div(kiters, per)
+                if (gemm_splitk_ws_bytes(d.N, m_tiles, d.batch, splits) <= d.splitk_ws_bytes) {   // one slice per k-slice
                     p.splits = splits;
                     p.kiters_per_split = per;
                     p.counters = reinterpret_cast<unsigned*>(d.splitk_ws);
-                    p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(d.splitk_ws) + counters_bytes);
+                    p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(d.splitk_ws) + kSplitkCounterBytes);
                 }
             }
         }

@@ -38,11 +38,6 @@ template <> struct Vec2<__nv_bfloat16> {
     }
 };
 
-__device__ __forceinline__ float silu_grad(float z) {
-    const float s = __fdividef(1.0f, 1.0f + __expf(-z));
-    return s * (1.0f + z * (1.0f - s));
-}
-
 // Per-group accumulation into shared memory in a fixed order, so that the statistics are bit-identical from run to run:
 // lanes of a warp that hold the same group add up with shuffles (a tree over a contiguous run, else in lane order), the
 // run's first lane adds the result into its warp's slot, and group_acc_flush() adds the slots into s_a / s_b in warp

@@ -497,6 +497,78 @@ def layernorm_bwd(dy, x, gamma, stats, *, dx=None, accumulate=False, dx_dtype=to
 
 
 # ------------------------------------------------------------------------------------------------
+# parameter gradients (fine-tuning the UNet / CLIP weights): fp32 results, alpha = 1 / loss scale
+# ------------------------------------------------------------------------------------------------
+def conv2d_wgrad(x, geo, dy, *, ksize=3, stride=1, pad=1, alpha=1.0, out=None):
+    """dW [cout][cin][k][k] fp32 of a k x k convolution (k = 1 or 3, symmetric padding `pad`) from its NHWC input
+    x [geo.rows][cin] and output gradient dy [n*oh*ow][cout], both 16-bit (cb_conv_wgrad)."""
+    assert x.stride(1) == 1 and dy.stride(1) == 1 and x.dtype == dy.dtype and x.shape[0] == geo.rows
+    cin, cout = x.shape[1], dy.shape[1]
+    L = _L()
+    col_b, sk_b = ctypes.c_longlong(0), ctypes.c_longlong(0)
+    _lib.check(L.cb_conv_wgrad_ws_bytes(geo.n, geo.h, geo.w, cin, cout, ksize, stride, pad, ctypes.byref(col_b),
+                                        ctypes.byref(sk_b)), "cb_conv_wgrad_ws_bytes")
+    col = torch.empty(col_b.value // 2, dtype=x.dtype, device=x.device) if col_b.value else None
+    ws = _splitk_workspace(x.device)
+    if out is None:
+        out = torch.empty(cout, cin, ksize, ksize, dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == (cout, cin, ksize, ksize)
+    _lib.check(L.cb_conv_wgrad(_p(x), x.stride(0), _p(dy), dy.stride(0), _dt(x), geo.n, geo.h, geo.w, cin, cout, ksize,
+                               stride, pad, float(alpha), _p(out), _p(col), _p(ws), ws.numel(), _st()), "cb_conv_wgrad")
+    return out
+
+
+def linear_wgrad(x, dy, *, alpha=1.0, out=None):
+    """dW[N][K] = alpha * dy[M][N]^T @ x[M][K] in fp32: one cb_gemm with both operands read MN-major."""
+    M, K = x.shape
+    N = dy.shape[1]
+    assert dy.shape[0] == M and x.stride(1) == 1 and dy.stride(1) == 1 and x.dtype == dy.dtype
+    if out is None:
+        out = torch.empty(N, K, dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.stride(1) == 1
+    d = GemmDesc()
+    d.M, d.N, d.K, d.batch, d.ab_dtype = N, K, M, 1, _dt(x)
+    d.A, d.lda, d.a_major = dy.data_ptr(), dy.stride(0), CB_MAJOR_MN
+    d.B, d.ldb, d.b_major = x.data_ptr(), x.stride(0), CB_MAJOR_MN
+    d.D, d.d_dtype, d.ldd = out.data_ptr(), CB_F32, out.stride(0)
+    d.alpha = alpha
+    _gemm(d, "cb_gemm(linear_wgrad)")
+    return out
+
+
+def colsum(x, *, groups=1, alpha=1.0, out=None):
+    """out[g][c] = alpha * sum of x's rows of group g (groups equal runs of rows), fp32 [groups][C] (cb_colsum)."""
+    assert x.dim() == 2 and x.stride(1) == 1
+    rows, C = x.shape
+    if out is None:
+        out = torch.empty(groups, C, dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() == groups * C
+    _lib.check(_L().cb_colsum(_p(x), _dt(x), x.stride(0), _p(out), rows, C, groups, float(alpha), _st()), "cb_colsum")
+    return out
+
+
+def groupnorm_affine_bwd(dy, x, geo, gamma, beta, stats, *, groups=32, silu=False, alpha=1.0):
+    """(dgamma, dbeta) fp32 [C] of a GroupNorm (fused with SiLU when silu) from the forward's saved statistics."""
+    C = x.shape[1]
+    dg = torch.empty(C, dtype=torch.float32, device=x.device)
+    db = torch.empty_like(dg)
+    _lib.check(_L().cb_groupnorm_affine_bwd(_p(dy), _dt(dy), _p(x), _dt(x), _p(gamma), _p(beta), _p(stats.mean),
+                                            _p(stats.rstd), _p(dg), _p(db), geo.n, geo.hw, C, groups, 1 if silu else 0,
+                                            float(alpha), _st()), "cb_groupnorm_affine_bwd")
+    return dg, db
+
+
+def layernorm_affine_bwd(dy, x, stats, *, alpha=1.0):
+    """(dgamma, dbeta) fp32 [C] of a LayerNorm from the forward's saved statistics."""
+    M, C = x.shape
+    dg = torch.empty(C, dtype=torch.float32, device=x.device)
+    db = torch.empty_like(dg)
+    _lib.check(_L().cb_layernorm_affine_bwd(_p(dy), _dt(dy), _p(x), _dt(x), _p(stats.mean), _p(stats.rstd), _p(dg),
+                                            _p(db), M, C, float(alpha), _st()), "cb_layernorm_affine_bwd")
+    return dg, db
+
+
+# ------------------------------------------------------------------------------------------------
 # pointwise
 # ------------------------------------------------------------------------------------------------
 def axpby(x, a=1.0, y=None, b=0.0, *, out=None, out_dtype=None):
@@ -703,6 +775,19 @@ def embedding_gather(ids, table):
     out = torch.empty(n, table.shape[1], dtype=torch.float32, device=table.device)
     _lib.check(_L().cb_embedding_gather(_p(ids), _p(table), _p(out), n, table.shape[1], table.shape[0], _st()),
                "cb_embedding_gather")
+    return out
+
+
+def embedding_bwd(ids, dout, num_rows, *, alpha=1.0, out=None):
+    """Gradient [num_rows][D] fp32 of embedding_gather: row v = alpha * the sum of dout's rows whose id is v, added in
+    token order; rows no id selects are zero (cb_embedding_bwd)."""
+    n, D = ids.numel(), dout.shape[1]
+    assert dout.dtype == torch.float32 and dout.stride(1) == 1 and dout.shape[0] == n and ids.dtype == torch.int64
+    if out is None:
+        out = torch.zeros(num_rows, D, dtype=torch.float32, device=dout.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == (num_rows, D)
+    _lib.check(_L().cb_embedding_bwd(_p(ids.contiguous()), _p(dout), dout.stride(0), _p(out), n, D, num_rows,
+                                     float(alpha), _st()), "cb_embedding_bwd")
     return out
 
 

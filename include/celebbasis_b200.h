@@ -435,6 +435,47 @@ int cb_pack_conv_weight(const float* w, void* out, int o_dtype, int cout, int ci
 int cb_convert_f32(const float* x, void* out, int o_dtype, long long n, float scale, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Parameter gradients for fine-tuning the UNet and the CLIP text encoder (`unfreeze_model`, ddpm.py:1450-1452): the
+ * weight, bias and affine gradients torch.autograd computes for the reference's nn.Conv2d / nn.Linear / GroupNorm32 /
+ * nn.LayerNorm / nn.Embedding.  Outputs are fp32; alpha scales every result (e.g. 1 / the static loss scale).  Every sum
+ * is taken in a fixed order: bit-reproducible from run to run.
+ * cb_conv_wgrad: dW[co][ci][ky][kx] = alpha * sum_{n,oh,ow} dy[n][oh][ow][co] * x[n][oh*s+ky-pad][ow*s+kx-pad][ci]
+ *   (zero outside the image) for k x k kernels, k = 1 or 3, stride s, symmetric padding; x is NHWC [N*H*W][ldx], dy
+ *   [N*OH*OW][lddy], both of `dtype` (CB_F16 / CB_BF16); dW is written in the nn.Parameter layout [cout][cin][k][k].
+ *   cin, cout, ldx and lddy must be multiples of 8 and the pointers 16-byte aligned (CB_ERR_ALIGN otherwise): pad the
+ *   channels with zeros and slice the result.  One cb_gemm launch (M = cout, N = cin*k*k, K = N*OH*OW, both operands
+ *   MN-major) over `col`, the taps of x gathered in the parameter's column order by one more launch; a 1x1 stride-1
+ *   unpadded convolution (and so a linear layer, x = [rows][in]) reads x directly and needs no col.  The k-loop is split
+ *   into a number of slices that depends on the shape and the device's SM count only, reduced in slice order through
+ *   splitk_ws (the cb_gemm split-K workspace: zero-filled before its first use, every call leaves its counters zero).
+ * cb_conv_wgrad_ws_bytes: host-only; the bytes of `col` (0: not used) and of splitk_ws (0: not used) that cb_conv_wgrad
+ *   needs for a geometry (CB_ERR_ARG if cb_conv_wgrad would refuse the geometry).
+ * cb_colsum: out[g][c] = alpha * sum of rows [g*rows/groups, (g+1)*rows/groups) of x[rows][ldx], column c < C (x of
+ *   any dtype).  groups = 1: a bias gradient; groups = images: the per-image sum of a pixel gradient (the gradient of a
+ *   ResBlock's emb_layers output, openaimodel.py:262-266 `h = h + emb_out`); a [B][T*D] view of the CLIP embedding
+ *   gradient: the position-embedding gradient (modules.py:295-296).
+ * cb_groupnorm_affine_bwd / cb_layernorm_affine_bwd: dgamma[c] = alpha * sum dz*xh, dbeta[c] = alpha * sum dz over all
+ *   rows, xh = (x - mean) * rstd from the forward's saved statistics ([N][G] / one per row), dz = dy, or
+ *   dy * silu'(xh*gamma + beta) with act_silu bit 0 (GroupNorm fused with SiLU).  Either output may be NULL.
+ * cb_embedding_bwd: dtable[v] = alpha * sum of the rows dout[i] (row pitch ld) of the tokens i with ids[i] == v, added in
+ *   token order; ids are clamped to [0, V) like cb_embedding_gather; rows of ids that do not occur are not written.
+ * ------------------------------------------------------------------------------------------- */
+int cb_conv_wgrad_ws_bytes(int N, int H, int W, int cin, int cout, int k, int stride, int pad, long long* col_bytes,
+                           long long* splitk_bytes);
+int cb_conv_wgrad(const void* x, long long ldx, const void* dy, long long lddy, int dtype, int N, int H, int W, int cin,
+                  int cout, int k, int stride, int pad, float alpha, float* dW, void* col, void* splitk_ws,
+                  long long splitk_ws_bytes, void* stream);
+int cb_colsum(const void* x, int x_dtype, long long ldx, float* out, long long rows, int C, int groups, float alpha,
+              void* stream);
+int cb_groupnorm_affine_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, const float* gamma,
+                            const float* beta, const float* mean, const float* rstd, float* dgamma, float* dbeta, int N,
+                            int HW, int C, int G, int act_silu, float alpha, void* stream);
+int cb_layernorm_affine_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, const float* mean,
+                            const float* rstd, float* dgamma, float* dbeta, int M, int C, float alpha, void* stream);
+int cb_embedding_bwd(const long long* ids, const float* dout, long long ld, float* dtable, int n, int D, int V,
+                     float alpha, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Device-side data path (SURVEY 8f-2): the pixel work of FaceIdDatasetStyleGAN3.__getitem__
  * (ldm/data/face_id.py:526-532 transform chain, :451-470 _add_bg, :598-644).  Random draws stay on the host.
  * cb_face_augment: uint8 [B][H][W][3] -> RandomHorizontalFlip, ColorJitter (ops in the drawn order, torchvision tensor
